@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — masks/sec of the PSALM inference hot path (PSALM.eval_seg) on B200.
+"""bench.py — masks/sec of the PSALM inference hot path (PSALM.eval_seg) on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 Workload (BASELINE.json configs[1]): COCO-panoptic prompt with 134 class names, 1024x1024 image,
@@ -9,9 +9,8 @@ Workload (BASELINE.json configs[1]): COCO-panoptic prompt with 134 class names, 
 of that architecture (no checkpoint or dataset is reachable offline).  One step = eval_seg on one
 batch of B images per GPU; masks/sec = images/sec x 100.  Default B = 4 (BASELINE.json configs[3] shards
 32 images over 8 GPUs = 4 per GPU; configs[1] does not fix a batch size): the library GEMMs of the Phi
-prefill run at M = 4 x 920 tokens instead of 920 and the step is 27 % cheaper per image than at B = 1
-(measured: B = 1 / 2 / 4 / 8 -> 12.2 K / 15.0 K / 16.7 K / 16.9 K masks/s; `--batch 1` reproduces the
-single-image latency of the reference's eval scripts, 8.2 ms).
+prefill run at M = 4 x 920 tokens instead of 920; `--batch 1` reproduces the single-image latency of the
+reference's eval scripts.
 
   value : inputs (normalised image, sequence plan) already resident in HBM, device-timed (CUDA events),
           CUDA-graph replay of the network + task heads, includes the post-processing (and its one small D2H copy).
@@ -55,7 +54,7 @@ def env_int(name, default):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -97,8 +96,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 700 W card)"
 
 
 MSDA_KERNEL = "msda_encoder_fused_kernel"   # the L1-gather kernel (auto); the TMA-tile kernel (impl 3) is slower, DESIGN.md
@@ -145,8 +144,8 @@ def tensor_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))
-    return 1590.0
+        return d.get("bf16_tflops_sustained", d.get("bf16_tflops", 989.0))
+    return 989.0    # H100 SXM data sheet, dense BF16
 
 
 def msda_algorithmic_bytes(B, S=21504, M=8, D=32, L=3, P=4, e_val=2, e_ow=2):
@@ -243,6 +242,54 @@ def run_reference(args, rank, world):
 
 
 # ------------------------------------------------------------------------------------------------
+DUMP_CAP = 1 << 18          # values per dumped array; larger outputs are stored as a fixed, seeded sample
+
+
+def dump_outputs(dirname, results, num_queries, max_instances):
+    """Write what the last timed step returned to its caller (PSALM.post_process results, one dict per image) as
+    DIR/img<b>_<field>.npy in float32 (float64 for integer fields, exactly; masks as 0 / 1).  Arrays above DUMP_CAP values keep a fixed
+    sample of DUMP_CAP positions (seeded by the array size, so two builds sample the same positions); the flat indices
+    go to <name>_idx.npy.  Panoptic segment records are stored as num_queries rows [id, isthing, category_id] (at most one
+    segment per query), unused rows -1, so that the array has the same shape whatever the number of segments; instance
+    fields likewise have max_instances rows, rows beyond the image's instances filled with -1."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    arrays = {}
+
+    def add(name, t):
+        t = t.detach().cpu()
+        a = t.float().numpy() if t.is_floating_point() or t.dtype == torch.bool else t.double().numpy()
+        if a.size > DUMP_CAP:
+            idx = np.sort(np.random.default_rng(a.size).choice(a.size, DUMP_CAP, replace=False))
+            arrays[name + "_idx"] = idx.astype(np.float64)
+            a = a.reshape(-1)[idx]
+        arrays[name] = a
+    for b, r in enumerate(results):
+        for key, val in r.items():
+            if torch.is_tensor(val):
+                add("img%d_%s" % (b, key), val)
+            elif key == "panoptic_seg":
+                ids, info = val
+                add("img%d_panoptic_ids" % b, ids)
+                seg = torch.full((num_queries, 3), -1.0, dtype=torch.float64)
+                for i, d in enumerate(info):
+                    seg[i] = torch.tensor([d["id"], int(d["isthing"]), d["category_id"]], dtype=torch.float64)
+                add("img%d_panoptic_segments" % b, seg)
+            elif hasattr(val, "get_fields"):
+                for f, v in val.get_fields().items():
+                    v = getattr(v, "tensor", v)
+                    if torch.is_tensor(v):
+                        v = v.detach().cpu()
+                        v = v.float() if v.is_floating_point() or v.dtype == torch.bool else v.double()
+                        pad = v.new_full((max_instances - v.shape[0],) + tuple(v.shape[1:]), -1)
+                        add("img%d_%s_%s" % (b, key, f), torch.cat([v, pad]))
+    total = sum(a.nbytes for a in arrays.values())
+    if total > 64 << 20:
+        raise RuntimeError("--dump-outputs: %d bytes exceed the 64 MB budget" % total)
+    for name, a in arrays.items():
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
+
 def timed_device_steps(step, K, W, barrier):
     for _ in range(W):
         step()
@@ -287,13 +334,18 @@ def run_ours(args, rank, world, local_rank):
     plan_d = model.make_plan(inp["input_ids"], inp["attention_mask"], (IMG, IMG), inp["class_name_ids"],
                              inp["cls_indices"], inp["class_name_embedding_indices"]).to(dev)
 
+    last = {}
+
     def step_device():
         out = model.forward_core(images_d, plan_d) if args.no_graph else model.forward_core_graphed(images_d, plan_d)
-        return model.post_process(out, (IMG, IMG), inp["seg_info"])
+        last["results"] = model.post_process(out, (IMG, IMG), inp["seg_info"])
+        return last["results"]
 
     sampler = ClockSampler(local_rank)
     sampler.start()
     ms_total = timed_device_steps(step_device, K, W, barrier)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["results"], model.num_queries, model.test_topk_per_image)
     # outputs of the timed configuration (graph replay at batch B), kept for the parity / accuracy checks below
     out_timed = None
     if not args.no_graph:
@@ -566,6 +618,8 @@ def main():
     ap.add_argument("--acc-images", type=int, default=0,
                     help="held images per rank scored against the oracle (0 = 16 images divided over the ranks, at least 2)")
     ap.add_argument("--no-graph", action="store_true", help="launch kernels eagerly instead of replaying a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the results of the last timed step as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     rank, world, local_rank = env_int("RANK", 0), env_int("WORLD_SIZE", 1), env_int("LOCAL_RANK", 0)
     if args.impl == "reference":

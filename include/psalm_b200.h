@@ -1,5 +1,5 @@
 /*
- * psalm_b200 — C ABI of the B200-native PSALM inference hot path.
+ * psalm_b200 — C ABI of the PSALM inference hot path for H100 (sm_90a).
  *
  * Plain pointers and sizes only (no torch / ATen types).  Every entry point
  *   - takes DEVICE pointers unless the parameter name ends in `_host`,
@@ -9,7 +9,7 @@
  *      Python caller swallows every exception — ops/modules/ms_deform_attn.py:117; we never do.)
  *
  * Reference interfaces each entry point replaces are cited per function as
- * (path relative to /root/reference/psalm/model/…:line).
+ * (path relative to psalm/model/… of the reference repository:line).
  */
 #ifndef PSALM_B200_H_
 #define PSALM_B200_H_
@@ -36,7 +36,7 @@ enum {
 
 int psalm_abi_version(void);
 const char* psalm_last_error(void);
-/* compute capability the library was compiled for (100 => sm_100a) */
+/* compute capability the library was compiled for (90 => sm_90a) */
 int psalm_compiled_arch(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -117,9 +117,9 @@ int psalm_set_attention_impl(int impl);
 /* Causal prefill attention of the LLM (third-party PhiAttention eager path; call site
  * language_model/llava_phi.py:1354-1363).  qkv [B,T,3,nh,hd] with rotary already applied
  * (psalm_rotary_inplace); key_valid [B,T] uint8 (attention_mask) or NULL; out [B,T,nh*hd].
- * fp32 softmax as in the reference.  16-bit storage, head_dim 64, 256 <= T <= 2048: tcgen05 + TMEM kernel
- * (128-query tiles, S and O accumulators in tensor memory); otherwise the mma.sync flash kernel; fp32
- * storage: SIMT kernel.  psalm_set_causal_impl: 0 = auto, 1 = mma.sync, 2 = tcgen05 (error if unsupported). */
+ * fp32 softmax as in the reference.  16-bit storage: mma.sync flash kernel (head_dim 32 / 64); fp32 storage: SIMT
+ * kernel.  psalm_set_causal_impl: 0 = auto, 1 = mma.sync, 2 = long-sequence tensor-core kernel (the tensor-memory
+ * kernel of sm_100a; on sm_90a all three select the mma.sync flash kernel). */
 int psalm_set_causal_impl(int impl);
 int psalm_causal_attention(const void* qkv, const uint8_t* key_valid, void* out, int B, int T, int nh,
                            int hd, int dtype, void* stream);
@@ -152,8 +152,8 @@ int psalm_cross_attention(const void* q, const void* k, const void* v, const uin
  * feats^T < 0) packed 32 keys / word + row_open; the logits are never written. */
 int psalm_mask_bits_fused(const void* mask_embed, const void* feats, uint32_t* bits, uint8_t* row_open, int B,
                           int Q, int P, int C, int dtype, void* stream);
-/* Implementation selector of psalm_mask_logits for 16-bit storage: 0 = auto (tcgen05 + TMEM kernel for
- * P >= 8192, warp-level mma.sync below), 1 = mma.sync, 2 = tcgen05. */
+/* Implementation selector of psalm_mask_logits for 16-bit storage: 0 = auto (wgmma GEMM of psalm_linear_fused per image
+ * for P >= 8192, P % 256 == 0, Q <= 128; warp-level mma.sync below), 1 = mma.sync, 2 = wgmma wherever P % 256 == 0. */
 int psalm_set_mask_proj_impl(int impl);
 int psalm_mask_logits(const void* mask_embed, const void* feats, void* out, int B, int Q, int P, int C,
                       int dtype, int out_dtype, void* stream);
@@ -224,8 +224,9 @@ int psalm_postproc_fused_crop(const void* logits, const void* probsT_f16, const 
  *   row_open  [B,Lq] != 0: ignore the mask for that row (fully blocked rows attend everywhere, :647), or NULL
  *   workspace: psalm_masked_cross_attention_workspace_bytes(B, Lq, Lk) bytes (split-K partials), may be NULL if 0
  * ------------------------------------------------------------------------------------------ */
-/* implementation selector: 0 = auto (tcgen05 + TMEM kernel, csrc/xattn_tc5.cu), 1 = warp-level mma.sync kernel
- * (csrc/xattn_tma.cu), 2 = tcgen05.  Both are fed by TMA. */
+/* implementation selector: 0 = auto (per-head flash kernel below 2048 keys, the TMA-fed warp-level mma.sync kernel of
+ * csrc/xattn_tma.cu above), 1 = the TMA-fed kernel at every key count, 2 = same as 1 on sm_90a (the slot of the
+ * sm_100a tensor-memory kernel). */
 int psalm_set_cross_impl(int impl);
 size_t psalm_masked_cross_attention_workspace_bytes(int B, int Lq, int Lk);
 int psalm_masked_cross_attention(const void* q, const void* k, const void* v, long long kv_row_stride,
@@ -263,7 +264,7 @@ int psalm_patchify(const void* images, void* patches, const float* mean, const f
                    int H, int W, int patch, int in_dtype, int out_dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Linear layer with a fused epilogue (tcgen05 + TMEM accumulators, operands through TMA; csrc/gemm_tc5.cu):
+ * Linear layer with a fused epilogue (wgmma, register accumulators, operands and results through TMA; csrc/gemm_wgmma.cu):
  *   out = epilogue(a · wᵀ + bias), 16-bit storage (PSALM_BF16 / PSALM_F16), fp32 accumulation.
  * Replaces the library GEMM + the separate elementwise pass of
  *   epilogue 1: Swin `Mlp.fc1` followed by the exact-erf `nn.GELU` (multimodal_encoder/swin_trans.py:37-44);

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — generates tests/golden/* by running the UNMODIFIED reference
-(/root/reference, via oracle/ref_shims.py) in the build container.  The reference cannot travel to
+(a reference checkout, via oracle/ref_shims.py) in the build container.  The reference cannot travel to
 the GPU box, so its outputs are committed as small fixtures together with this script.
 
     python oracle/gen_golden.py manifest      # state-dict key/shape manifest from the reference constructors

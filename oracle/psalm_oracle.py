@@ -3,7 +3,7 @@ the reference `PSALM.eval_seg` path.  Only tests/, `__graft_entry__.smoke()` and
 cpu_baseline / `--impl reference` legs may import this module; nothing under psalm_b200/ does.
 
 Every function cites the reference lines it restates.  Abbreviations (relative to
-/root/reference/psalm/model/):
+psalm/model/ of the reference):
   LP   = language_model/llava_phi.py
   SWIN = multimodal_encoder/swin_trans.py
   PROJ = multimodal_projector/builder.py

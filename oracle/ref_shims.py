@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE — import shims that let the *unmodified* reference (`/root/reference`,
+"""TEST INFRASTRUCTURE — import shims that let the *unmodified* reference (a reference checkout named by PSALM_REFERENCE_ROOT,
 zamling/PSALM) run on CPU in the build container.  Used only by `oracle/gen_golden.py` (fixture
 generation) and by `tests/test_oracle_vs_reference.py` (skipped when the reference is absent, e.g.
 on the GPU box).  Nothing in `psalm_b200/` imports this file.
@@ -19,7 +19,7 @@ import types
 import torch
 import torch.nn.functional as F
 
-REFERENCE_ROOT = os.environ.get("PSALM_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("PSALM_REFERENCE_ROOT", "")
 
 _FAKE_ROOTS = ("detectron2", "pycocotools", "panopticapi", "timm", "fvcore", "addict",
                "MultiScaleDeformableAttention", "shortuuid", "iopath", "matplotlib")
@@ -30,7 +30,7 @@ _SUBMODULES = ("transforms", "detection_utils", "mask", "comm", "data", "utils",
 
 
 def reference_available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "psalm"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "psalm"))
 
 
 class _AutoMock(types.ModuleType):

@@ -7,9 +7,8 @@
 //                      registers (9 warps x 16 rows), single-pass softmax, relative-position bias and
 //                      the shift mask applied on the accumulators, window gather / zero padding / cyclic
 //                      shift resolved once per CTA into a token table in shared memory.
-// Both use warp-level mma.sync.m16n8k16 with ldmatrix operand fetch.  (tcgen05 is reserved for the
-// GEMM-shaped mask projection — these tiles are 144- or 64-wide with per-element bias / mask work in
-// the accumulators, which TMEM round trips would not speed up; see DESIGN.md.)
+// Both use warp-level mma.sync.m16n8k16 with ldmatrix operand fetch: these tiles are 144- or 64-wide with
+// per-element bias / mask work in the accumulators (see DESIGN.md).
 #include <type_traits>
 
 #include <cooperative_groups.h>
@@ -762,11 +761,11 @@ static int launch_flash(const Policy& pol, AttnDims dm, int hd, float* workspace
   if (hd == 32) {
     if (kg2) launch_flash_kg<T, 32, Policy, 2>(pol, dm, workspace, st);
     else launch_flash_kg<T, 32, Policy, 1>(pol, dm, workspace, st);
-    if (dm.splits > 1) flash_combine_kernel<Policy, 32><<<148 * 2, 256, 0, st>>>(pol, dm, workspace);
+    if (dm.splits > 1) flash_combine_kernel<Policy, 32><<<132 * 2, 256, 0, st>>>(pol, dm, workspace);
   } else if (hd == 64) {
     if (kg2) launch_flash_kg<T, 64, Policy, 2>(pol, dm, workspace, st);
     else launch_flash_kg<T, 64, Policy, 1>(pol, dm, workspace, st);
-    if (dm.splits > 1) flash_combine_kernel<Policy, 64><<<148 * 2, 256, 0, st>>>(pol, dm, workspace);
+    if (dm.splits > 1) flash_combine_kernel<Policy, 64><<<132 * 2, 256, 0, st>>>(pol, dm, workspace);
   } else {
     set_error("%s: head_dim %d unsupported by the tensor-core path", what, hd);
     return PSALM_E_UNSUPPORTED;
@@ -818,10 +817,10 @@ static int launch_window(const void* qkv, const void* qkv_bias, const float* rel
     window_mma_kernel<T, HPC><<<grid, 288, smem, st>>>((const T*)qkv, (const T*)qkv_bias, rel, (T*)out, H, W, Hp,   \
                                                       Wp, shift, nh, C, nWx, nW);                                 \
   } while (0)
-  // enough CTAs for >= 2 waves of 148 SMs x 3 CTAs, otherwise prefer deeper per-CTA pipelining
+  // enough CTAs for >= 2 waves of 132 SMs x 3 CTAs, otherwise prefer deeper per-CTA pipelining
   const long long windows = (long long)B * nW;
   if (nh % 4 == 0 && windows * (nh / 4) >= 600) WIN(4);
-  else if (nh % 2 == 0 && windows * (nh / 2) >= 148) WIN(2);
+  else if (nh % 2 == 0 && windows * (nh / 2) >= 132) WIN(2);
   else WIN(1);
 #undef WIN
   return check_launch("window_mma_kernel");

@@ -11,7 +11,7 @@
 //   CrossPolicy   Mask2Former masked cross-attention / query self-attention
 //                 (transformer_decoder/mask2former_transformer_decoder.py:93-105, 35-45) with a packed
 //                 bit mask (1 = blocked) and the "fully blocked row attends everywhere" rule (:647).
-// Split-K over the keys (partials + combine) keeps 100-query problems on all 148 SMs.
+// Split-K over the keys (partials + combine) keeps 100-query problems on all 132 SMs.
 #include "common.cuh"
 
 namespace psalm {
@@ -284,10 +284,10 @@ static int launch_attn(const Policy& pol, AttnDims dm, int zdim, int hd, float* 
   PSALM_REQUIRE(dm.splits == 1 || workspace != nullptr, "%s: split-K needs a workspace", what);
   if (hd == 32) {
     attn_simt_kernel<Policy, 32><<<grid, kNT, 0, st>>>(pol, dm, workspace);
-    if (dm.splits > 1) attn_combine_kernel<Policy, 32><<<148 * 4, 256, 0, st>>>(pol, dm, workspace);
+    if (dm.splits > 1) attn_combine_kernel<Policy, 32><<<132 * 4, 256, 0, st>>>(pol, dm, workspace);
   } else if (hd == 64) {
     attn_simt_kernel<Policy, 64><<<grid, kNT, 0, st>>>(pol, dm, workspace);
-    if (dm.splits > 1) attn_combine_kernel<Policy, 64><<<148 * 4, 256, 0, st>>>(pol, dm, workspace);
+    if (dm.splits > 1) attn_combine_kernel<Policy, 64><<<132 * 4, 256, 0, st>>>(pol, dm, workspace);
   } else {
     set_error("%s: head_dim %d unsupported (32 or 64)", what, hd);
     return PSALM_E_UNSUPPORTED;
@@ -363,9 +363,6 @@ int mma_cross_attention(const void*, const void*, const void*, const uint32_t*, 
 int mma_window_attention(const void*, const void*, const float*, void*, int, int, int, int, int, int, int,
                          cudaStream_t);
 extern int g_splitk_mode;
-bool tc5_causal_ok(int B, int T_, int nh, int hd, int dtype);
-int tc5_causal_attention(const void*, const uint8_t*, void*, int, int, int, int, int, cudaStream_t);
-static int g_causal_impl = 0;   // 0 auto, 1 mma.sync, 2 tcgen05
 static int g_attn_impl = 0;  // 0 = auto (tensor cores for 16-bit storage), 1 = force the fp32 SIMT kernels
 }  // namespace psalm
 
@@ -379,8 +376,8 @@ extern "C" int psalm_set_attention_impl(int impl) {
 }
 
 extern "C" int psalm_set_causal_impl(int impl) {
-  PSALM_REQUIRE(impl >= 0 && impl <= 2, "set_causal_impl: 0 (auto), 1 (mma.sync) or 2 (tcgen05)");
-  g_causal_impl = impl;
+  PSALM_REQUIRE(impl >= 0 && impl <= 2, "set_causal_impl: 0 (auto), 1 (mma.sync) or 2 (long-sequence tensor-core kernel); all "
+                                        "select the mma.sync flash kernel on sm_90a");
   return PSALM_OK;
 }
 
@@ -414,11 +411,6 @@ extern "C" int psalm_window_attention(const void* qkv, const void* qkv_bias, con
 extern "C" int psalm_causal_attention(const void* qkv, const uint8_t* key_valid, void* out, int B, int T_,
                                       int nh, int hd, int dtype, void* stream) {
   PSALM_REQUIRE(qkv && out, "causal_attention: null pointer");
-  if (g_attn_impl == 0 && g_causal_impl == 2)
-    return tc5_causal_attention(qkv, key_valid, out, B, T_, nh, hd, dtype, (cudaStream_t)stream);
-  // tcgen05 kernel: 128-query tiles; below ~2 tiles per head the 64-row mma.sync kernel fills the GPU better
-  if (g_attn_impl == 0 && g_causal_impl == 0 && T_ >= 256 && tc5_causal_ok(B, T_, nh, hd, dtype))
-    return tc5_causal_attention(qkv, key_valid, out, B, T_, nh, hd, dtype, (cudaStream_t)stream);
   if (dtype != PSALM_F32 && g_attn_impl == 0 && (hd == 32 || hd == 64))
     return mma_causal_attention(qkv, key_valid, out, B, T_, nh, hd, dtype, (cudaStream_t)stream);
   AttnDims dm{B, nh, T_, T_, 1, 1.0f / sqrtf((float)hd)};
@@ -436,13 +428,13 @@ extern "C" int psalm_rotary_inplace(void* qkv, const float* cos_t, const float* 
   PSALM_REQUIRE(rd % 2 == 0 && rd <= hd, "rotary: bad rotary dim %d (head dim %d)", rd, hd);
   if (dtype != PSALM_F32 && (rd / 2) % 8 == 0 && hd % 8 == 0) {
     const long long nv = (long long)B * T_ * 2 * nh * (rd / 16);
-    const int vb = (int)((nv + 255) / 256 < 148 * 16 ? (nv + 255) / 256 : 148 * 16);
+    const int vb = (int)((nv + 255) / 256 < 132 * 16 ? (nv + 255) / 256 : 132 * 16);
     if (dtype == PSALM_BF16) rotary_vec_kernel<__nv_bfloat16><<<vb > 0 ? vb : 1, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)qkv, cos_t, sin_t, B, T_, nh, hd, rd);
     else rotary_vec_kernel<__half><<<vb > 0 ? vb : 1, 256, 0, (cudaStream_t)stream>>>((__half*)qkv, cos_t, sin_t, B, T_, nh, hd, rd);
     return check_launch("rotary_vec_kernel");
   }
   const long long n = (long long)B * T_ * 2 * nh * (rd / 2);
-  const int blocks = (int)((n + 255) / 256 < 148 * 16 ? (n + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16);
   DISPATCH_T(dtype, {
     rotary_kernel<T><<<blocks > 0 ? blocks : 1, 256, 0, (cudaStream_t)stream>>>((T*)qkv, cos_t, sin_t, B, T_, nh, hd, rd);
   });

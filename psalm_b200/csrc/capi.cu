@@ -13,4 +13,4 @@ void set_error(const char* fmt, ...) {
 
 extern "C" int psalm_abi_version(void) { return PSALM_ABI_VERSION; }
 extern "C" const char* psalm_last_error(void) { return psalm::g_err; }
-extern "C" int psalm_compiled_arch(void) { return 100; }
+extern "C" int psalm_compiled_arch(void) { return 90; }

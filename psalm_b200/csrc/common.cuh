@@ -1,4 +1,4 @@
-// Shared helpers for the psalm_b200 CUDA kernels (sm_100a).
+// Shared helpers for the psalm_b200 CUDA kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -75,14 +75,10 @@ template <> __device__ __forceinline__ uint32_t pack2<__half>(float lo, float hi
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// packed fp32 FMA (Blackwell FFMA2): acc.xy += v.xy * w
+// acc.xy += v.xy * w, one rounding per lane (Hopper has no packed fp32 FMA)
 __device__ __forceinline__ void ffma2(float2& acc, const float2 v, const float w) {
-  unsigned long long a = *reinterpret_cast<unsigned long long*>(&acc);
-  const unsigned long long b = *reinterpret_cast<const unsigned long long*>(&v);
-  const float2 ww = make_float2(w, w);
-  const unsigned long long c = *reinterpret_cast<const unsigned long long*>(&ww);
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a) : "l"(b), "l"(c));
-  acc = *reinterpret_cast<float2*>(&a);
+  acc.x = fmaf(v.x, w, acc.x);
+  acc.y = fmaf(v.y, w, acc.y);
 }
 
 // 16-byte vector of CH elements of T (CH = 4 for fp32, 8 for 16-bit types), as fp32 lanes

@@ -119,7 +119,7 @@ extern "C" int psalm_kv_cache_write(const void* qkv, void* kcache, void* vcache,
   PSALM_REQUIRE(hd % (16 / (int)dtype_size(dtype)) == 0, "kv_cache_write: head_dim %d not a multiple of 16 bytes", hd);
   cudaStream_t st = (cudaStream_t)stream;
   const long long n = (long long)B * T_ * 2 * nh * (hd / (16 / (int)dtype_size(dtype)));
-  const int blocks = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+  const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
   if (dtype == PSALM_F32) kv_cache_write_kernel<float><<<blocks, 256, 0, st>>>((const float*)qkv, (float*)kcache, (float*)vcache, block_table, start_pos, B, T_, nh, hd, page_size, max_pages);
   else if (dtype == PSALM_F16) kv_cache_write_kernel<__half><<<blocks, 256, 0, st>>>((const __half*)qkv, (__half*)kcache, (__half*)vcache, block_table, start_pos, B, T_, nh, hd, page_size, max_pages);
   else if (dtype == PSALM_BF16) kv_cache_write_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>((const __nv_bfloat16*)qkv, (__nv_bfloat16*)kcache, (__nv_bfloat16*)vcache, block_table, start_pos, B, T_, nh, hd, page_size, max_pages);

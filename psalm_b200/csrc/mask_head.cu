@@ -154,16 +154,15 @@ __global__ void attn_mask_bits_kernel(const T* __restrict__ logits, uint32_t* __
 }  // namespace psalm
 
 namespace psalm {
-int tc5_mask_proj(const void* me, const void* feats, void* out, int B, int Q, int P, int dtype, cudaStream_t st);
-static int g_mask_proj_impl = 0;   // 0 auto, 1 mma.sync, 2 tcgen05
 int mma_mask_proj(const void* me, const void* feats, void* out, uint32_t* bits, uint8_t* row_open, int B, int Q, int P,
                   int dtype, cudaStream_t st);
+static int g_mask_proj_impl = 0;   // 0 auto, 1 mma.sync, 2 wgmma GEMM where it applies
 }
 
 using namespace psalm;
 
 extern "C" int psalm_set_mask_proj_impl(int impl) {
-  PSALM_REQUIRE(impl >= 0 && impl <= 2, "set_mask_proj_impl: 0 (auto), 1 (mma.sync) or 2 (tcgen05)");
+  PSALM_REQUIRE(impl >= 0 && impl <= 2, "set_mask_proj_impl: 0 (auto), 1 (mma.sync) or 2 (wgmma where P %% 256 == 0)");
   g_mask_proj_impl = impl;
   return PSALM_OK;
 }
@@ -182,9 +181,18 @@ extern "C" int psalm_mask_logits(const void* mask_embed, const void* feats, void
                                  int C, int dtype, int out_dtype, void* stream) {
   PSALM_REQUIRE(mask_embed && feats && out, "mask_logits: null pointer");
   PSALM_REQUIRE(out_dtype == dtype || out_dtype == PSALM_F32, "mask_logits: out dtype must be F32 or the input dtype");
-  if (dtype != PSALM_F32 && out_dtype == dtype && C == 256 && Q <= 128 &&
-      (g_mask_proj_impl == 2 || (g_mask_proj_impl == 0 && P >= 8192)))
-    return tc5_mask_proj(mask_embed, feats, out, B, Q, P, dtype, (cudaStream_t)stream);   // tcgen05 + TMEM
+  // large maps: per image one wgmma GEMM out[b] = mask_embed[b] (Q x C, TMA zero-fills rows Q..127 of the tile) ·
+  // feats[b]ᵀ (P x C), both operands K-major as stored (csrc/gemm_wgmma.cu)
+  if (dtype != PSALM_F32 && out_dtype == dtype && C == 256 && Q <= 128 && P % 256 == 0 &&
+      (g_mask_proj_impl == 2 || (g_mask_proj_impl == 0 && P >= 8192))) {
+    const size_t es = dtype_size(dtype);
+    for (int b = 0; b < B; ++b) {
+      const int rc = psalm_linear_fused((const char*)mask_embed + (size_t)b * Q * C * es, C, (const char*)feats + (size_t)b * P * C * es,
+                                        nullptr, (char*)out + (size_t)b * Q * P * es, Q, P, C, 0, 0, dtype, stream);
+      if (rc != PSALM_OK) return rc;
+    }
+    return PSALM_OK;
+  }
   if (dtype != PSALM_F32 && out_dtype == dtype && C == 256 && Q <= 112 && P % 2 == 0)
     return mma_mask_proj(mask_embed, feats, out, nullptr, nullptr, B, Q, P, dtype, (cudaStream_t)stream);
   dim3 grid((P + 127) / 128, (Q + 31) / 32, B);
@@ -203,12 +211,12 @@ extern "C" int psalm_bilinear_tokens(const void* in, void* out, int B, int Hi, i
   PSALM_REQUIRE(in && out, "bilinear_tokens: null pointer");
   PSALM_REQUIRE(out_dtype == dtype || out_dtype == PSALM_F32, "bilinear_tokens: out dtype must be F32 or the input dtype");
   const long long n = (long long)B * Ho * Wo * C;
-  const int blocks = (int)((n + 255) / 256 < 148 * 32 ? (n + 255) / 256 : 148 * 32);
+  const int blocks = (int)((n + 255) / 256 < 132 * 32 ? (n + 255) / 256 : 132 * 32);
   cudaStream_t st = (cudaStream_t)stream;
   if (out_dtype == dtype && C % (dtype == PSALM_F32 ? 4 : 8) == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(out) & 15) == 0) {
     const long long nv = n / (dtype == PSALM_F32 ? 4 : 8);
-    const int vb = (int)((nv + 255) / 256 < 148 * 16 ? (nv + 255) / 256 : 148 * 16);
+    const int vb = (int)((nv + 255) / 256 < 132 * 16 ? (nv + 255) / 256 : 132 * 16);
 #define BLV(T) bilinear_tokens_vec_kernel<T><<<vb > 0 ? vb : 1, 256, 0, st>>>((const T*)in, (T*)out, B, Hi, Wi, Ho, Wo, C, accumulate)
     if (dtype == PSALM_F32) BLV(float);
     else if (dtype == PSALM_F16) BLV(__half);

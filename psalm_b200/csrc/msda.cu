@@ -1,4 +1,4 @@
-// Multi-scale deformable attention forward for sm_100a.
+// Multi-scale deformable attention forward for sm_90a.
 //
 // Replaces ms_deformable_im2col_gpu_kernel (reference ops/src/cuda/ms_deform_im2col_cuda.cuh:243-304,
 // one thread per output scalar, scalar loads, queries walked in linear order).  Design here:
@@ -436,7 +436,7 @@ static int launch_msda(const void* value, const int64_t* shapes, const int64_t* 
 
   if (!vec_ok) {
     const long long n = (long long)B * Lq * M * D;
-    const int blocks = (int)((n + 255) / 256 < 148 * 32 ? (n + 255) / 256 : 148 * 32);
+    const int blocks = (int)((n + 255) / 256 < 132 * 32 ? (n + 255) / 256 : 132 * 32);
     msda_scalar_kernel<TV, TL><<<blocks > 0 ? blocks : 1, 256, 0, st>>>(
         (const TV*)value, (const TL*)loc, (const TL*)w, (TV*)out, sdev, stdev, lv, n, S, M, D, L, Lq, P,
         pix_stride, head_stride, batch_stride);

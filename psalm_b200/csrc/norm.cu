@@ -291,7 +291,7 @@ static int launch_gn(const void* x, const void* pre_bias, const void* w, const v
   groupnorm_finalize_kernel<<<(n_bg + 127) / 128, 128, 0, st>>>(part, mean_rstd, n_bg, n_part,
                                                               (double)N * (C / groups), eps);
   const long long n4 = (long long)B * N * C / 4;
-  const int blocks = (int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   groupnorm_apply_kernel<T><<<blocks > 0 ? blocks : 1, 256, 0, st>>>((const T*)x, (const T*)pre_bias, mean_rstd, (const T*)w, (const T*)b,
                                                                      (T*)y, B, N, C, groups, relu);
   return check_launch("groupnorm_tokens");

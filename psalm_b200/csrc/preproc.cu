@@ -57,7 +57,7 @@ static int launch_patchify(const void* img, void* out, const float* mean, const 
                            int W, int ps, int out_dtype, cudaStream_t st) {
   const int Wh = (H + ps - 1) / ps, Ww = (W + ps - 1) / ps;
   const long long n = (long long)B * Wh * Ww * Cin * ps;
-  const int blocks = (int)((n + 255) / 256 < 148 * 16 ? (n + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16);
 #define PSALM_PATCHIFY(TO)                                                                                       \
   patchify_kernel<TI, TO, 4><<<blocks, 256, 0, st>>>((const TI*)img, (TO*)out, mean, stdv, B, Cin, H, W, Wh, Ww)
   if (out_dtype == PSALM_F32) PSALM_PATCHIFY(float);

@@ -29,7 +29,7 @@
 //     small second kernel.
 // Tensor work is warp-level mma.sync.m16n8k16: at head_dim 32 the contraction is 2 k-steps, the kernel is bound by
 // the exp2 / mask ALU work on the score fragments (MUFU: 58.7 M exp2 at HW = 16384, B = 4 = 12.9 us of the SFU pipe),
-// which tcgen05 would not remove (DESIGN.md section 4).
+// which larger tensor-core instructions would not remove (DESIGN.md section 4).
 #include <cuda.h>
 
 #include <type_traits>
@@ -500,7 +500,7 @@ static int xa_sm_count() {
   static PerDevice cache;
   const int d = PerDevice::dev();
   if (cache.first() || cache.v[d] == 0) cudaDeviceGetAttribute(&cache.v[d], cudaDevAttrMultiProcessorCount, d);
-  return cache.v[d] > 0 ? cache.v[d] : 148;
+  return cache.v[d] > 0 ? cache.v[d] : 132;
 }
 
 static int xa_splits(int B, int Lk) {
@@ -515,11 +515,7 @@ static int xa_splits(int B, int Lk) {
   return (steps + per - 1) / per;                   // drop empty trailing splits
 }
 
-// tcgen05 + TMEM kernel (xattn_tc5.cu)
-int tc5_cross_workspace_bytes(int B, int Lq, int Lk, size_t* bytes);
-int tc5_cross_attention(const void*, const void*, const void*, long long, const uint32_t*, const uint8_t*, void*, float*, size_t,
-                        int, int, int, int, cudaStream_t);
-static int g_cross_impl = 0;   // 0 auto, 1 warp-level mma.sync + TMA, 2 tcgen05
+static int g_cross_impl = 0;   // 0 auto, 1 / 2 always the TMA-fed kernel of this file
 // per-head flash kernel of attn_mma.cu (row-strided K / V views supported)
 int mma_cross_attention(const void*, const void*, const void*, const uint32_t*, const uint8_t*, void*, float*, int, int, int, int,
                         int, int, int, cudaStream_t, int kv_ld);
@@ -527,7 +523,7 @@ constexpr int kSmallLk = 2048;   // below this many keys the problem is launch /
                                  // few key tiles per CTA wins (measured, tools/bench_cross.py)
 static int small_splits(int B, int Lk) {
   const int ctas = B * 8 * 2;
-  int want = (2 * 148 + ctas - 1) / ctas;
+  int want = (2 * 132 + ctas - 1) / ctas;
   const int cap = (Lk + 255) / 256;
   if (want > cap) want = cap;
   if (want > 16) want = 16;
@@ -538,7 +534,7 @@ static int small_splits(int B, int Lk) {
 
 extern "C" int psalm_set_cross_impl(int impl) {
   if (impl < 0 || impl > 2) {
-    psalm::set_error("psalm_set_cross_impl: 0 (auto), 1 (mma.sync) or 2 (tcgen05)");
+    psalm::set_error("psalm_set_cross_impl: 0 (auto), 1 or 2 (TMA-fed mma.sync kernel at every key count)");
     return PSALM_E_ARG;
   }
   psalm::g_cross_impl = impl;
@@ -549,9 +545,6 @@ extern "C" size_t psalm_masked_cross_attention_workspace_bytes(int B, int Lq, in
   using namespace psalm;
   const int s = xa_splits(B, Lk);
   size_t a = s > 1 ? (size_t)B * s * xa::NH * xa::ROWS * (xa::HD + 2) * sizeof(float) : 0;
-  size_t t = 0;
-  tc5_cross_workspace_bytes(B, Lq, Lk, &t);
-  if (t > a) a = t;
   const int ss = small_splits(B, Lk);
   const size_t u = ss > 1 ? (size_t)B * xa::NH * ss * Lq * (xa::HD + 2) * sizeof(float) : 0;
   return a > u ? a : u;      // any implementation may be selected at run time
@@ -565,7 +558,7 @@ extern "C" int psalm_masked_cross_attention(const void* q, const void* k, const 
   PSALM_REQUIRE(q && k && v && out, "masked_cross_attention: null pointer");
   PSALM_REQUIRE(nh == xa::NH && hd == xa::HD, "masked_cross_attention: needs 8 heads x 32 (got %d x %d)", nh, hd);
   PSALM_REQUIRE(dtype == PSALM_BF16 || dtype == PSALM_F16, "masked_cross_attention: 16-bit storage only");
-  PSALM_REQUIRE(Lq >= 1 && Lq <= xa::ROWS, "masked_cross_attention: 1..%d queries (got %d)", xa::ROWS, Lq);   // tcgen05: <= 128
+  PSALM_REQUIRE(Lq >= 1 && Lq <= xa::ROWS, "masked_cross_attention: 1..%d queries (got %d)", xa::ROWS, Lq);
   PSALM_REQUIRE(B >= 1 && B <= 65535 && Lk >= 1, "masked_cross_attention: bad B / Lk");
   PSALM_REQUIRE(kv_row_stride >= xa::C && kv_row_stride % 8 == 0, "masked_cross_attention: K/V row stride %lld", kv_row_stride);
   PSALM_REQUIRE(((uintptr_t)k & 15) == 0 && ((uintptr_t)v & 15) == 0 && ((uintptr_t)q & 15) == 0 && ((uintptr_t)out & 3) == 0,
@@ -575,8 +568,6 @@ extern "C" int psalm_masked_cross_attention(const void* q, const void* k, const 
     const int ss = small_splits(B, Lk);
     return mma_cross_attention(q, k, v, mask_bits, row_open, out, workspace, B, Lq, Lk, nh, hd, ss, dtype, st, (int)kv_row_stride);
   }
-  if (g_cross_impl != 1)
-    return tc5_cross_attention(q, k, v, kv_row_stride, mask_bits, row_open, out, workspace, workspace_bytes, B, Lq, Lk, dtype, st);
   XaParams p;
   p.q = q; p.bits = mask_bits; p.row_open = row_open; p.out = out;
   p.B = B; p.Lq = Lq; p.Lk = Lk; p.W32 = (Lk + 31) / 32;

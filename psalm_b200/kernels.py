@@ -1,5 +1,5 @@
 """Torch-tensor wrappers over the C ABI (include/psalm_b200.h).  PyTorch is used only for device
-memory, streams and library GEMMs; every function here launches hand-written sm_100a kernels and
+memory, streams and library GEMMs; every function here launches hand-written sm_90a kernels and
 raises (never falls back) when the library is missing or an argument is wrong."""
 import torch
 
@@ -103,9 +103,9 @@ def causal_attention(qkv, key_valid, B, T, nh, hd):
 
 
 def pick_splits(B, nh, Lq, Lk):
-    """Split-K factor so that a 100-query problem still fills ~2 waves of 148 SMs."""
+    """Split-K factor so that a 100-query problem still fills ~2 waves of 132 SMs."""
     ctas = B * nh * ((Lq + 63) // 64)
-    want = max(1, (2 * 148 + ctas - 1) // ctas)
+    want = max(1, (2 * 132 + ctas - 1) // ctas)
     # every CTA walks at least 4 key tiles of 64 (two per key group) so that the partial-result traffic stays small
     # <= 16: the split-K partials are reduced inside one thread-block cluster (distributed shared memory)
     return int(max(1, min(want, (Lk + 255) // 256, 16)))
@@ -365,7 +365,7 @@ def linear_fused_supported(x, weight, epilogue, rows_per_image=0):
 
 @_on_device
 def linear_fused(x, weight, bias, epilogue, rows_per_image=0):
-    """epilogue(x @ weight.T + bias) on the tcgen05 tensor cores (csrc/gemm_tc5.cu).  x [..., K] (rows contiguous),
+    """epilogue(x @ weight.T + bias) on the Hopper tensor cores (wgmma, csrc/gemm_wgmma.cu).  x [..., K] (rows contiguous),
     weight [N, K].  epilogue: "bias", "gelu_erf" (Swin Mlp.fc1 + nn.GELU, swin_trans.py:37-44) or "head_major"
     (MSDeformAttn value_proj stored [B, N/32, rows_per_image, 32], ms_deform_attn.py:95-99)."""
     _chk(weight, "linear_fused.weight")

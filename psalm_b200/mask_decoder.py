@@ -2,7 +2,7 @@
 
 Mirrors `MultiScaleMaskedTransformerDecoderForOPTPreTrain.forward_woconcat`
 (reference transformer_decoder/mask2former_transformer_decoder.py:596-693) and
-`forward_prediction_heads` (:695-762).  B200-first differences:
+`forward_prediction_heads` (:695-762).  Differences from the reference:
   * masked cross-attention and the 100x100 query self-attention are one fused kernel each
     (psalm_cross_attention) working on a PACKED BIT mask (1 bit / key, shared by the 8 heads) instead of
     nn.MultiheadAttention with a float -inf mask of shape [B*8, 100, HW] and materialised probabilities;

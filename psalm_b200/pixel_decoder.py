@@ -2,7 +2,7 @@
 
 Mirrors `MSDeformAttnPixelDecoder.forward_features` (reference mask_decoder/Mask2Former_Simplify/
 modeling/pixel_decoder/msdeformattn.py:268-315), the encoder (:136-164, :89-95, :57-66) and
-`MSDeformAttn.forward` (ops/modules/ms_deform_attn.py:82-124).  B200-first differences:
+`MSDeformAttn.forward` (ops/modules/ms_deform_attn.py:82-124).  Differences from the reference:
   * feature maps are [B, H*W, C] (C contiguous): 1x1 convolutions are plain GEMMs and mask_features
     comes out K-major for the mask-projection kernel;
   * sampling_offsets and attention_weights are ONE GEMM (288 outputs); softmax, reference points,

@@ -94,8 +94,10 @@ def test_cross_attention_with_bit_mask(dt, Lq, Lk, splits):
                                         (2, 100, 27889, 768), (3, 37, 100, 256), (1, 112, 389, 768), (2, 1, 33, 256),
                                         (5, 100, 6400, 768), (1, 100, 31, 256)])
 def test_masked_cross_attention_tma(impl, dt, B, Lq, Lk, ld):
-    """The TMA-fed masked cross-attention kernels (tcgen05 + TMEM: csrc/xattn_tc5.cu; warp-level mma.sync:
-    csrc/xattn_tma.cu) vs the torch restatement: packed bit masks, fully blocked rows that re-open, fully open rows,
+    """The masked cross-attention kernels (auto: per-head flash kernel below 2048 keys, TMA-fed warp-level mma.sync
+    kernel of csrc/xattn_tma.cu above; selectors 1 and 2 (the Blackwell tensor-memory kernel's slot, "tcgen05" in the
+    ids): the TMA-fed kernel at every key count) vs the torch restatement: packed bit masks, fully blocked rows that
+    re-open, fully open rows,
     ragged key counts (tail tile), row-strided K / V views of a fused projection buffer, single-CTA and split-K grids,
     and the no-mask case."""
     from psalm_b200 import _lib
@@ -207,8 +209,9 @@ def test_mask_bits_fused_and_mma_logits(dt, P, attn_impl):
 @pytest.mark.parametrize("dt", ["bf16", "f16"])
 @pytest.mark.parametrize("B,Q,P", [(1, 100, 8192), (2, 100, 4096 + 96), (1, 128, 65536), (3, 7, 130)])
 def test_mask_projection_tcgen05(dt, B, Q, P, attn_impl):
-    """tcgen05 + TMEM mask projection (csrc/mask_proj_tc5.cu) vs the fp32 restatement; also vs the mma.sync
-    kernel (bit-for-bit is not required: both accumulate in fp32 but in different orders)."""
+    """Large-P mask projection selector (2; the slot of the Blackwell tensor-memory kernel, on H100 the wgmma GEMM of
+    csrc/gemm_wgmma.cu for P % 256 == 0, the mma.sync / generic kernels otherwise) vs the fp32 restatement; also
+    vs the mma.sync selector (1) within the same tolerance (both accumulate in fp32, in different orders)."""
     if attn_impl == "simt":
         pytest.skip("independent of the attention implementation switch")
     from psalm_b200 import _lib
@@ -219,17 +222,23 @@ def test_mask_projection_tcgen05(dt, B, Q, P, attn_impl):
     try:
         _lib.check(_lib.lib().psalm_set_mask_proj_impl(2), "set_mask_proj_impl")
         out = kernels.mask_logits(me.cuda(), f.cuda())
+        _lib.check(_lib.lib().psalm_set_mask_proj_impl(1), "set_mask_proj_impl")
+        out1 = kernels.mask_logits(me.cuda(), f.cuda())
         torch.cuda.synchronize()
     finally:
         _lib.lib().psalm_set_mask_proj_impl(0)
     _close(out, ref, dt)
+    _close(out1, ref, dt)
+    auto = kernels.mask_logits(me.cuda(), f.cuda())
+    assert torch.equal(auto, out if P >= 8192 else out1)
 
 
 @pytest.mark.parametrize("dt", ["f16", "bf16"])
 @pytest.mark.parametrize("T,padded", [(64, False), (130, True), (257, False), (900, True), (1100, False), (1100, True), (2048, False)])
 @pytest.mark.parametrize("impl", [1, 2])
 def test_causal_attention_impls(dt, T, padded, impl):
-    """mma.sync flash kernel (1) and tcgen05 + TMEM kernel (2) against the fp32 restatement."""
+    """Causal attention selectors 1 (mma.sync flash kernel) and 2 (the long-sequence tensor-core slot; on H100 the same
+    flash kernel) against the fp32 restatement, up to the 2048-token prefill."""
     from psalm_b200 import _lib
     torch.manual_seed(T + impl)
     B, nh, hd = 2, 3, 64

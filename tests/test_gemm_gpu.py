@@ -1,4 +1,4 @@
-"""Fused-epilogue linear layers on the tcgen05 tensor cores (csrc/gemm_tc5.cu) against a plain PyTorch fp32 evaluation of
+"""Fused-epilogue linear layers on the Hopper tensor cores (wgmma, csrc/gemm_wgmma.cu) against a plain PyTorch fp32 evaluation of
 the same op on the same 16-bit inputs: Swin `Mlp.fc1` + exact-erf GELU (swin_trans.py:37-44), MSDeformAttn `value_proj`
 stored head-major (ms_deform_attn.py:95-99), plain bias.  Tolerance: the result is rounded once to 16 bits (rel 2^-9 bf16 /
 2^-12 fp16) on top of fp32 accumulation; asserted as |err| <= rtol * |ref| + atol with atol tied to the output scale."""

@@ -43,7 +43,7 @@ def main():
         row_open = torch.zeros(B, Lq, dtype=torch.uint8).cuda()
         nbytes = B * (2 * Lk * C * 2 + Lq * Lk // 8 + 2 * Lq * C * 2)
         from psalm_b200 import _lib
-        runs = (("tcgen05_tma", 2, lambda: kernels.masked_cross_attention(q, k, v, bits, row_open, nh)),
+        runs = (("tma_auto", 0, lambda: kernels.masked_cross_attention(q, k, v, bits, row_open, nh)),
                 ("mma_tma", 1, lambda: kernels.masked_cross_attention(q, k, v, bits, row_open, nh)),
                 ("per_head_mma", 0, lambda: kernels.cross_attention(q, kc, vc, bits, row_open, nh)))
         for name, impl, fn in runs:

@@ -1,4 +1,4 @@
-"""Time the fused-epilogue tcgen05 linear kernel (csrc/gemm_tc5.cu) next to the library path it replaces (cuBLAS GEMM +
+"""Time the fused-epilogue wgmma linear kernel (csrc/gemm_wgmma.cu) next to the library path it replaces (cuBLAS GEMM +
 stand-alone GELU pass / transposing copy) on the shapes of the bench step (B images of 1024^2).
 usage: B=4 python tools/bench_gemm.py"""
 import json

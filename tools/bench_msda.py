@@ -30,9 +30,9 @@ def timeit(fn, iters=20, warmup=5, flush=None):
 
 
 def load_reference_op():
-    """The reference's own CUDA op built for sm_100 by baseline/build_ref_msda.py (None if it was not built)."""
+    """The reference's own CUDA op built for sm_90a by oracle/build_ref_msda.py (None if it was not built)."""
     import importlib.util
-    so = os.path.join(ROOT, "baseline", "_ref", "MultiScaleDeformableAttention.so")
+    so = os.path.join(ROOT, "oracle", "_ref", "MultiScaleDeformableAttention.so")
     if not os.path.exists(so):
         return None
     spec = importlib.util.spec_from_file_location("MultiScaleDeformableAttention", so)

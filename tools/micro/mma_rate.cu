@@ -1,5 +1,5 @@
-// Micro-benchmark: issue rate of warp-level mma.sync.m16n8k16 (bf16 -> fp32) and MUFU.EX2 on sm_100a, per SM.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/mma_rate tools/micro/mma_rate.cu
+// Micro-benchmark: issue rate of warp-level mma.sync.m16n8k16 (bf16 -> fp32) and MUFU.EX2 on sm_90a (H100), per SM.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/mma_rate tools/micro/mma_rate.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
