@@ -293,6 +293,32 @@ int psalm_patch_merge_layernorm(const void* x, const void* weight, const void* b
 int psalm_region_pool(const void* tokens, const float* points, const int* region_image, void* out, int B, int h, int w,
                       int C, int R, int P, int dtype, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * COCO run-length encoding of binary masks (SURVEY.md section 8 f1; csrc/rle.cu).  The contract is pycocotools'
+ * maskApi.c, restated: runs in column-major pixel order j = x*H + y, the first run counts background (may be 0), counts
+ * uint32.  A pixel is foreground iff its value is non-zero.  Encoding takes three calls; the caller reads run_off[n] after
+ * the first and byte_off[n] after the second to size `ends` and `chars`.
+ *   masks [n,H,W] row-major contiguous (dtype PSALM_F32 or PSALM_U8), or mask_ptrs [n] = device address of each [H,W]
+ *   mask (masks is then ignored); workspace: psalm_rle_workspace_bytes(n, H, W) bytes.
+ * psalm_rle_count (rleEncode's run count, rleArea, rleToBbox): run_off [n+1] int64 = exclusive prefix sum of the run
+ *   counts, area [n] int64 = sum of the odd runs, bbox [n,4] float64 = [x, y, w, h] of the foreground, zeros when empty.
+ *   The dense masks are read once; later calls read a 1-bit column-major copy in the workspace.
+ * psalm_rle_runs (rleEncode): ends [run_off[n]] uint32 = end of every run (cumulative counts, mask after mask);
+ *   byte_off [n+1] int64 = exclusive prefix sum of the string lengths of rleToString.
+ * psalm_rle_strings (rleToString): chars [byte_off[n]], the strings of the masks back to back, no terminators.
+ * psalm_rle_decode (rleFrString + rleDecode): chars / byte_off as above -> out [n,H,W] uint8 0/1; workspace ends
+ *   [byte_off[n]] uint32, nruns [n] int64.
+ * ------------------------------------------------------------------------------------------ */
+size_t psalm_rle_workspace_bytes(int n, int H, int W);
+int psalm_rle_count(const void* masks, const uint64_t* mask_ptrs, void* workspace, int64_t* run_off, int64_t* area,
+                    double* bbox, int n, int H, int W, int dtype, void* stream);
+int psalm_rle_runs(const void* workspace, const int64_t* run_off, uint32_t* ends, int64_t* byte_off, int n, int H, int W,
+                   void* stream);
+int psalm_rle_strings(const uint32_t* ends, const int64_t* run_off, const int64_t* byte_off, uint8_t* chars, int n,
+                      void* stream);
+int psalm_rle_decode(const uint8_t* chars, const int64_t* byte_off, uint32_t* ends, int64_t* nruns, uint8_t* out, int n,
+                     int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

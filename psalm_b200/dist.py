@@ -135,3 +135,26 @@ def reduce_sum(tensors, device):
             dist.all_reduce(t, op=dist.ReduceOp.SUM)
         outs.append(t)
     return outs
+
+
+def gather_rle(chars, offsets):
+    """Ragged gather of the device form of RLE-encoded masks (psalm_b200/rle.py): chars uint8 [bytes] (the strings back
+    to back) and offsets int64 [n+1] of this rank -> list over ranks, in rank order, of (chars, offsets).  The per-rank
+    sizes are gathered first; the payloads then travel padded to the largest rank.  Identity without a process group."""
+    if not (dist.is_initialized() and dist.get_world_size() > 1):
+        return [(chars, offsets)]
+    world = dist.get_world_size()
+    dev = chars.device
+    sizes = torch.tensor([chars.numel(), offsets.numel()], dtype=torch.int64, device=dev)
+    all_sizes = [torch.empty_like(sizes) for _ in range(world)]
+    dist.all_gather(all_sizes, sizes)
+    all_sizes = torch.stack(all_sizes).cpu().tolist()
+    out = []
+    for k, t in enumerate((chars, offsets)):
+        top = max(1, max(s[k] for s in all_sizes))
+        pad = torch.zeros(top, dtype=t.dtype, device=dev)
+        pad[:t.numel()] = t.reshape(-1)
+        g = torch.empty(world * top, dtype=t.dtype, device=dev)
+        dist.all_gather_into_tensor(g, pad)
+        out.append([g[r * top:r * top + all_sizes[r][k]] for r in range(world)])
+    return list(zip(out[0], out[1]))

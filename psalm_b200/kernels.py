@@ -469,3 +469,63 @@ def paged_decode_attention(qkv, kcache, vcache, block_table, seq_lens):
     _lib.check(rc, "psalm_paged_decode_attention")
     _count()
     return out
+
+
+def rle_encode(masks):
+    """COCO RLE of binary masks (csrc/rle.cu): `masks` is a [n,H,W] CUDA tensor or a list of [k,H,W] CUDA tensors sharing
+    H, W and dtype (float32, uint8 or bool; non-zero = foreground), encoded together in one batch.  Returns
+    dict(chars uint8 [bytes], offsets int64 [n+1], area int64 [n], bbox float64 [n,4]): mask i's rleToString string is
+    chars[offsets[i]:offsets[i+1]].  Two small device-to-host copies (run and byte totals) size the outputs."""
+    parts = [masks] if isinstance(masks, torch.Tensor) else list(masks)
+    for t in parts:
+        _chk(t, "rle_encode.masks")
+        if t.dim() != 3 or t.shape[1:] != parts[0].shape[1:] or t.dtype != parts[0].dtype or t.device != parts[0].device:
+            raise _lib.PsalmKernelError("rle_encode: masks are [n,H,W] tensors of one size, dtype and device")
+    dtype = parts[0].dtype
+    if dtype not in (torch.float32, torch.uint8, torch.bool):
+        raise _lib.PsalmKernelError("rle_encode: masks must be float32, uint8 or bool, got %s" % dtype)
+    dev = parts[0].device
+    _, H, W = parts[0].shape
+    n = sum(t.shape[0] for t in parts)
+    with torch.cuda.device(dev):
+        L = _lib.lib()
+        ptrs = None
+        if len(parts) > 1:   # one address per mask: the masks of several tensors are read in place
+            es = parts[0].element_size() * H * W
+            ptrs = torch.tensor([t.data_ptr() + k * es for t in parts for k in range(t.shape[0])], dtype=torch.int64).to(dev)
+        base = parts[0].view(torch.uint8) if dtype == torch.bool else parts[0]
+        ws = torch.empty(L.psalm_rle_workspace_bytes(n, H, W), dtype=torch.uint8, device=dev)
+        run_off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        area = torch.empty(n, dtype=torch.int64, device=dev)
+        bbox = torch.empty((n, 4), dtype=torch.float64, device=dev)
+        s = _lib.stream_ptr(dev)
+        _lib.check(L.psalm_rle_count(_lib.ptr(base), _lib.ptr(ptrs) if ptrs is not None else None, _lib.ptr(ws),
+                                     _lib.ptr(run_off), _lib.ptr(area), _lib.ptr(bbox), n, H, W,
+                                     _lib.F32 if dtype == torch.float32 else _lib.U8, s), "psalm_rle_count")
+        ends = torch.empty(int(run_off[n]), dtype=torch.int32, device=dev)            # device-to-host copy 1
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        _lib.check(L.psalm_rle_runs(_lib.ptr(ws), _lib.ptr(run_off), _lib.ptr(ends), _lib.ptr(offsets), n, H, W, s),
+                   "psalm_rle_runs")
+        chars = torch.empty(int(offsets[n]), dtype=torch.uint8, device=dev)           # device-to-host copy 2
+        _lib.check(L.psalm_rle_strings(_lib.ptr(ends), _lib.ptr(run_off), _lib.ptr(offsets), _lib.ptr(chars), n, s),
+                   "psalm_rle_strings")
+    _count(7)
+    return dict(chars=chars, offsets=offsets, area=area, bbox=bbox)
+
+
+@_on_device
+def rle_decode(chars, offsets, H, W):
+    """rleFrString + rleDecode (csrc/rle.cu): strings chars[offsets[i]:offsets[i+1]] (uint8 / int64 CUDA tensors) ->
+    uint8 [n,H,W] 0/1."""
+    _chk(chars, "rle_decode.chars")
+    _chk(offsets, "rle_decode.offsets")
+    if chars.dtype != torch.uint8 or offsets.dtype != torch.int64:
+        raise _lib.PsalmKernelError("rle_decode: chars uint8, offsets int64")
+    n = offsets.numel() - 1
+    ends = torch.empty(max(chars.numel(), 1), dtype=torch.int32, device=chars.device)
+    nruns = torch.empty(n, dtype=torch.int64, device=chars.device)
+    out = torch.empty((n, H, W), dtype=torch.uint8, device=chars.device)
+    _lib.check(_lib.lib().psalm_rle_decode(_lib.ptr(chars), _lib.ptr(offsets), _lib.ptr(ends), _lib.ptr(nruns), _lib.ptr(out),
+                                           n, H, W, _lib.stream_ptr(chars.device)), "psalm_rle_decode")
+    _count(2)
+    return out

@@ -55,9 +55,10 @@ class PendingSeg:
     under a side stream.  The tensors of the result live in the lane's static buffers: they stay valid until the next
     submission on the same lane."""
 
-    def __init__(self, model, out, image_hw, seg_info, boxes, done, hostvecs, thing_list, thresholds):
+    def __init__(self, model, out, image_hw, seg_info, boxes, done, hostvecs, thing_list, thresholds, mask_format="dense"):
         self.model, self.out, self.image_hw, self.seg_info, self.boxes = model, out, image_hw, seg_info, boxes
         self.done, self.hostvecs, self.thing_list, self.thresholds = done, hostvecs, thing_list, thresholds
+        self.mask_format = mask_format
 
     def result(self):
         m = self.model
@@ -66,9 +67,34 @@ class PendingSeg:
         keep = (getattr(m, "is_thing_list", None), m.object_mask_threshold, m.overlap_threshold)
         m.is_thing_list, (m.object_mask_threshold, m.overlap_threshold) = self.thing_list, self.thresholds
         try:
-            return m.post_process(self.out, self.image_hw, self.seg_info, self.boxes, hostvecs=self.hostvecs)
+            results = m.post_process(self.out, self.image_hw, self.seg_info, self.boxes, hostvecs=self.hostvecs)
         finally:
             m.is_thing_list, m.object_mask_threshold, m.overlap_threshold = keep
+        if self.mask_format == "rle":
+            attach_rle(results)
+        return results
+
+
+MASK_FORMATS = ("dense", "rle")
+
+
+def attach_rle(results):
+    """mask_format="rle": `instances.pred_masks_rle` = pycocotools RLE dicts of `instances.pred_masks` (same order) for
+    every result with instances.  The masks of all images of a size are encoded in one batch on the device."""
+    from . import rle
+    groups = {}
+    for r in results:
+        inst = r.get("instances")
+        if inst is not None:
+            m = inst.pred_masks
+            groups.setdefault((tuple(m.shape[1:]), m.dtype, m.device), []).append(inst)
+    for insts in groups.values():
+        dicts = rle.to_dicts(rle.encode_device([i.pred_masks for i in insts]))
+        pos = 0
+        for inst in insts:
+            k = inst.pred_masks.shape[0]
+            inst.pred_masks_rle = dicts[pos:pos + k]
+            pos += k
 
 
 class PSALMModel:
@@ -464,23 +490,32 @@ class PSALM:
     def eval_seg(self, input_ids=None, attention_mask=None, past_key_values=None, inputs_embeds=None, labels=None,
                  use_cache=None, output_attentions=None, output_hidden_states=None, images=None, return_dict=None,
                  seg_info=None, class_name_ids=None, class_name_embedding_indices=None, cls_indices=None,
-                 token_refer_id=None, refer_embedding_indices=None, is_thing_list=None, region_points=None, vp_images=None):
+                 token_refer_id=None, refer_embedding_indices=None, is_thing_list=None, region_points=None, vp_images=None,
+                 mask_format="dense"):
+        """`mask_format`: "dense" (default) returns the reference's results; "rle" adds `instances.pred_masks_rle`, the
+        COCO RLE dicts of `instances.pred_masks` encoded on the device (psalm_b200/rle.py), to every result with
+        instances - what a COCO evaluator consumes, without copying the dense masks to the host."""
         if self.panoptic_on:
             assert is_thing_list is not None, "is_thing_list need to be given"   # llava_phi.py:1337-1339
             self.is_thing_list = is_thing_list
         return self.eval_seg_async(region_points=region_points, vp_images=vp_images, input_ids=input_ids, attention_mask=attention_mask, images=images, seg_info=seg_info,
                                    class_name_ids=class_name_ids, class_name_embedding_indices=class_name_embedding_indices,
                                    cls_indices=cls_indices, token_refer_id=token_refer_id,
-                                   refer_embedding_indices=refer_embedding_indices, is_thing_list=is_thing_list).result()
+                                   refer_embedding_indices=refer_embedding_indices, is_thing_list=is_thing_list,
+                                   mask_format=mask_format).result()
 
     @torch.no_grad()
     def eval_seg_async(self, input_ids=None, attention_mask=None, images=None, seg_info=None, class_name_ids=None,
                        class_name_embedding_indices=None, cls_indices=None, token_refer_id=None,
-                       refer_embedding_indices=None, is_thing_list=None, lane=0, region_points=None, vp_images=None):
+                       refer_embedding_indices=None, is_thing_list=None, lane=0, region_points=None, vp_images=None,
+                       mask_format="dense"):
         """Submit one `eval_seg` call and return a `PendingSeg`; `.result()` gives what `eval_seg` returns.  `lane`
         selects an independent CUDA graph + static output buffers, so that a caller alternating lanes 0 / 1 can finish
         batch k (host merge, read-back) while the device already runs batch k+1.  `region_points`: optional per-sample
-        [K,256,2] sample points for <region> prompts (default: drawn like the reference, psalm_b200/region.py)."""
+        [K,256,2] sample points for <region> prompts (default: drawn like the reference, psalm_b200/region.py).
+        `mask_format`: see `eval_seg`; the encoding runs in `result()`."""
+        if mask_format not in MASK_FORMATS:
+            raise ValueError("mask_format must be one of %s, got %r" % (MASK_FORMATS, mask_format))
         if self.panoptic_on:
             assert is_thing_list is not None, "is_thing_list need to be given"   # llava_phi.py:1337-1339
             self.is_thing_list = is_thing_list
@@ -532,7 +567,8 @@ class PSALM:
         done = torch.cuda.Event()
         done.record(cur)
         return PendingSeg(self, out, tuple(images.shape[-2:]), seg_info, boxes, done, hostvecs,
-                          getattr(self, "is_thing_list", None), (self.object_mask_threshold, self.overlap_threshold))
+                          getattr(self, "is_thing_list", None), (self.object_mask_threshold, self.overlap_threshold),
+                          mask_format)
 
     def _fused_applies(self, image_hw, seg_info):
         """(fuse_post, boxes): fuse_post is True when every image takes the fused task-head kernel without crop / resize,
