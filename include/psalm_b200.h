@@ -124,6 +124,15 @@ int psalm_set_causal_impl(int impl);
 int psalm_causal_attention(const void* qkv, const uint8_t* key_valid, void* out, int B, int T, int nh,
                            int hd, int dtype, void* stream);
 
+/* Causal prefill of B prompt suffixes behind one shared, already cached prefix of P tokens (several prompts against one
+ * image: the prefix K / V are computed once).  qkv [B,T,3,nh,hd] with rotary applied at positions P + t; prefix_k,
+ * prefix_v head-major [nh, prefix_ld_rows, hd] (rows 0..P-1 used; the layout of a one-page KV cache), shared by all B
+ * sequences; key_valid [B,T] uint8 or NULL (all valid); out [B,T,nh*hd].  Query t of sequence b attends prefix keys 0..P-1
+ * and its own keys u <= t with key_valid[b,u] set; rows of padded queries are finite.  16-bit storage: mma.sync flash
+ * kernel (head_dim 32 / 64, 64 * ceil(P / 64) + T <= 8192); fp32 storage: SIMT kernel. */
+int psalm_prefix_causal_attention(const void* qkv, const void* prefix_k, const void* prefix_v, int P, int prefix_ld_rows,
+                                  const uint8_t* key_valid, void* out, int B, int T, int nh, int hd, int dtype, void* stream);
+
 /* Partial rotary embedding in place on q and k of qkv [B,T,3,nh,hd]; cos/sin [T, rd/2] fp32
  * (PhiRotaryEmbedding + apply_rotary_pos_emb on the first rd dims). */
 int psalm_rotary_inplace(void* qkv, const float* cos_t, const float* sin_t, int B, int T, int nh, int hd,
@@ -157,6 +166,14 @@ int psalm_mask_bits_fused(const void* mask_embed, const void* feats, uint32_t* b
 int psalm_set_mask_proj_impl(int impl);
 int psalm_mask_logits(const void* mask_embed, const void* feats, void* out, int B, int Q, int P, int C,
                       int dtype, int out_dtype, void* stream);
+/* The same two operations with the feature map of query set b at feats + b * feats_batch_stride elements
+ * (feats_batch_stride = P * C for [B,P,C] maps; 0 = one image's map serves all B query sets, the prompts of one image).
+ * psalm_mask_bits_fused / psalm_mask_logits are these entries with the dense stride.  At stride 0 the wgmma path of
+ * psalm_mask_logits is one GEMM with M = B * Q rows. */
+int psalm_mask_bits_fused_strided(const void* mask_embed, const void* feats, long long feats_batch_stride, uint32_t* bits,
+                                  uint8_t* row_open, int B, int Q, int P, int C, int dtype, void* stream);
+int psalm_mask_logits_strided(const void* mask_embed, const void* feats, long long feats_batch_stride, void* out, int B, int Q,
+                              int P, int C, int dtype, int out_dtype, void* stream);
 int psalm_bilinear_tokens(const void* in, void* out, int B, int Hi, int Wi, int Ho, int Wo, int C, int dtype,
                           int out_dtype, int accumulate, void* stream);
 int psalm_attn_mask_bits(const void* logits, uint32_t* bits, uint8_t* row_open, int rows, int P, int dtype,
@@ -232,6 +249,13 @@ size_t psalm_masked_cross_attention_workspace_bytes(int B, int Lq, int Lk);
 int psalm_masked_cross_attention(const void* q, const void* k, const void* v, long long kv_row_stride,
                                  const uint32_t* mask_bits, const uint8_t* row_open, void* out, float* workspace,
                                  size_t workspace_bytes, int B, int Lq, int Lk, int nh, int hd, int dtype, void* stream);
+/* Same, with row n of image b at base + b * kv_batch_stride + n * kv_row_stride elements; kv_batch_stride is 0 (one
+ * image's memory serves all B query sets) or a multiple of kv_row_stride.  psalm_masked_cross_attention is this entry
+ * with kv_batch_stride = Lk * kv_row_stride. */
+int psalm_masked_cross_attention_strided(const void* q, const void* k, const void* v, long long kv_row_stride,
+                                         long long kv_batch_stride, const uint32_t* mask_bits, const uint8_t* row_open,
+                                         void* out, float* workspace, size_t workspace_bytes, int B, int Lq, int Lk, int nh,
+                                         int hd, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Autoregressive decode of the LLM (chat path: psalm/serve/cli.py:89-96 -> PSALM.generate; single-token branch

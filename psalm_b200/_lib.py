@@ -56,6 +56,11 @@ SIGNATURES = {
     "psalm_set_cross_impl": ([_c_i], _c_i),
     "psalm_masked_cross_attention_workspace_bytes": ([_c_i] * 3, ctypes.c_size_t),
     "psalm_masked_cross_attention": ([_c_vp] * 3 + [ctypes.c_longlong] + [_c_vp] * 4 + [ctypes.c_size_t] + [_c_i] * 6 + [_c_vp], _c_i),
+    "psalm_masked_cross_attention_strided": ([_c_vp] * 3 + [ctypes.c_longlong] * 2 + [_c_vp] * 4 + [ctypes.c_size_t] + [_c_i] * 6
+                                             + [_c_vp], _c_i),
+    "psalm_mask_bits_fused_strided": ([_c_vp] * 2 + [ctypes.c_longlong] + [_c_vp] * 2 + [_c_i] * 5 + [_c_vp], _c_i),
+    "psalm_mask_logits_strided": ([_c_vp] * 2 + [ctypes.c_longlong] + [_c_vp] + [_c_i] * 6 + [_c_vp], _c_i),
+    "psalm_prefix_causal_attention": ([_c_vp] * 3 + [_c_i] * 2 + [_c_vp] * 2 + [_c_i] * 5 + [_c_vp], _c_i),
     "psalm_kv_cache_write": ([_c_vp] * 5 + [_c_i] * 7 + [_c_vp], _c_i),
     "psalm_paged_decode_attention": ([_c_vp, ctypes.c_longlong] + [_c_vp] * 5 + [_c_i] * 6 + [_c_vp], _c_i),
     "psalm_patchify": ([_c_vp] * 4 + [_c_i] * 7 + [_c_vp], _c_i),

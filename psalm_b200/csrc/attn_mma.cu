@@ -76,6 +76,7 @@ struct CausalMma {
   T* out;                    // [B,T,nh*hd]
   int T_, nh, hd;
   static constexpr bool kCausal = true;
+  static constexpr bool kPrefix = false;
   __device__ __forceinline__ const T* ptr(int which, int b, int h, int n, int d0) const {
     return qkv + (((size_t)b * T_ + n) * 3 + which) * nh * hd + h * hd + d0;
   }
@@ -108,10 +109,12 @@ struct CrossMma {
   T* out;
   int Lq, Lk, nh, hd, W32;
   int kv_ld;   // elements between consecutive K (and V) rows: nh * hd, or more for views of a fused projection buffer
+  long long kv_bstride;   // elements between the K (and V) rows of consecutive images: Lk * kv_ld, or 0 = one shared memory
   static constexpr bool kCausal = false;
+  static constexpr bool kPrefix = false;
   __device__ __forceinline__ const T* ptr(int which, int b, int h, int n, int d0) const {
     if (which == 0) return q + ((size_t)b * Lq + n) * nh * hd + h * hd + d0;
-    return (which == 1 ? k : v) + ((size_t)b * Lk + n) * kv_ld + h * hd + d0;
+    return (which == 1 ? k : v) + (size_t)b * kv_bstride + (size_t)n * kv_ld + h * hd + d0;
   }
   __device__ __forceinline__ size_t row_stride() const { return (size_t)kv_ld; }
   __device__ __forceinline__ uint4 load8(int which, int b, int h, int n, int d0) const {
@@ -131,6 +134,44 @@ struct CrossMma {
   }
   __device__ __forceinline__ void store(int b, int h, int n, int d, float v) const {
     out[((size_t)b * Lq + n) * nh * hd + h * hd + d] = from_f32<T>(v);
+  }
+};
+
+// Causal prefill of prompt suffixes behind a shared prefix: query t of sequence b attends the P prefix keys (head-major
+// [nh, ld_rows, hd], the same for every b) and its own keys u <= t.  The virtual key axis is [prefix padded to Pt tiles
+// of 64 | own keys], so that a 64-key tile is either all prefix (row stride hd) or all own keys (row stride 3 nh hd);
+// keys in [P, 64 Pt) are invalid keys.
+template <typename T>
+struct PrefixCausalMma {
+  const T* qkv;              // [B,T,3,nh,hd], rotary applied at positions P + t
+  const T *pk, *pv;          // [nh, ld_rows, hd]
+  const uint8_t* key_valid;  // [B,T] or null
+  T* out;                    // [B,T,nh*hd]
+  int T_, nh, hd, P, ld_rows, Pt;
+  static constexpr bool kCausal = true;
+  static constexpr bool kPrefix = true;   // the kernel's prefetch picks base and row stride per key tile
+  __device__ __forceinline__ const T* ptr(int which, int b, int h, int n, int d0) const {
+    return qkv + (((size_t)b * T_ + n) * 3 + which) * nh * hd + h * hd + d0;
+  }
+  __device__ __forceinline__ size_t row_stride() const { return (size_t)3 * nh * hd; }   // own keys
+  __device__ __forceinline__ uint4 load8(int which, int b, int h, int n, int d0) const {
+    return ldg16(ptr(which, b, h, n, d0));
+  }
+  __device__ __forceinline__ unsigned long long blocked(int b, int qi, int kt, unsigned long long kv) const {
+    if (kt < Pt) return kv;
+    const int d = qi - (kt - Pt) * 64;
+    const unsigned long long m = d >= 63 ? 0ull : (d < 0 ? ~0ull : (~0ull << (d + 1)));
+    return m | kv;
+  }
+  __device__ __forceinline__ bool key_invalid(int b, int kj) const {
+    if (kj < Pt * 64) return kj >= P;
+    return key_valid && !key_valid[(size_t)b * T_ + kj - Pt * 64];
+  }
+  __device__ __forceinline__ void store2(int b, int h, int n, int d, float v0, float v1) const {
+    *reinterpret_cast<uint32_t*>(out + ((size_t)b * T_ + n) * nh * hd + h * hd + d) = pack2<T>(v0, v1);
+  }
+  __device__ __forceinline__ void store(int b, int h, int n, int d, float v) const {
+    out[((size_t)b * T_ + n) * nh * hd + h * hd + d] = from_f32<T>(v);
   }
 };
 
@@ -163,7 +204,8 @@ __global__ void __launch_bounds__(128 * KG, KG == 2 ? 2 : 4) flash_mma_kernel(Po
   const int kt0 = sp * tps;
   int kt1 = kt0 + tps < ktiles ? kt0 + tps : ktiles;
   if (Policy::kCausal) {
-    const int e = (q0 + BQ - 1) / BK + 1;
+    int e = (q0 + BQ - 1) / BK + 1;
+    if constexpr (Policy::kPrefix) e += pol.Pt;
     kt1 = e < kt1 ? e : kt1;
   }
   // ---- Q tile -> smem -> A fragments in registers
@@ -211,6 +253,26 @@ __global__ void __launch_bounds__(128 * KG, KG == 2 ? 2 : 4) flash_mma_kernel(Po
   }
   const size_t tile_stride = (size_t)BK * pol.row_stride();
   auto prefetch = [&](int kt, int stage) {
+    if constexpr (Policy::kPrefix) {
+      // a prefix tile (shared head-major K / V, row stride HD) or a tile of the sequence's own keys (row stride 3 nh hd)
+      const bool pre = kt < pol.Pt;
+      const size_t rs = pre ? (size_t)HD : (size_t)3 * pol.nh * HD;
+      const T* kb = pre ? pol.pk + ((size_t)h * pol.ld_rows + (size_t)kt * BK) * HD : pol.ptr(1, b, h, (kt - pol.Pt) * BK, 0);
+      const T* vb = pre ? pol.pv + ((size_t)h * pol.ld_rows + (size_t)kt * BK) * HD : kb + (size_t)pol.nh * HD;
+      const int left = pre ? pol.P - kt * BK : pol.T_ - (kt - pol.Pt) * BK;
+#pragma unroll
+      for (int j = 0; j < NSLOT; ++j) {
+        const int i = tid + 128 * j;
+        const int row = i / (HD / 8), c8 = (i % (HD / 8)) * 8;
+        const int so = row * LD + c8;
+        const bool ok = row < left;
+        const size_t go = (size_t)row * rs + c8;
+        cp_async16(&KVg[(stage * 2 + 0) * BK * LD + so], ok ? kb + go : pol.qkv, ok ? 16 : 0);
+        cp_async16(&KVg[(stage * 2 + 1) * BK * LD + so], ok ? vb + go : pol.qkv, ok ? 16 : 0);
+      }
+      cp_async_commit();
+      return;
+    }
     const T* kt_base = kbase + (size_t)kt * tile_stride;
     const int left = dm.Lk - kt * BK;   // keys of this tile that exist
 #pragma unroll
@@ -786,17 +848,32 @@ int mma_causal_attention(const void* qkv, const uint8_t* key_valid, void* out, i
 
 int mma_cross_attention(const void* q, const void* k, const void* v, const uint32_t* bits, const uint8_t* row_open,
                         void* out, float* workspace, int B, int Lq, int Lk, int nh, int hd, int splits, int dtype,
-                        cudaStream_t st, int kv_ld) {
+                        cudaStream_t st, int kv_ld, long long kv_bstride) {
   if (kv_ld <= 0) kv_ld = nh * hd;
+  if (kv_bstride < 0) kv_bstride = (long long)Lk * kv_ld;
   AttnDims dm{B, nh, Lq, Lk, splits, 1.0f / sqrtf((float)hd)};
   if (dtype == PSALM_BF16) {
     using T = __nv_bfloat16;
-    CrossMma<T> pol{(const T*)q, (const T*)k, (const T*)v, bits, row_open, (T*)out, Lq, Lk, nh, hd, (Lk + 31) / 32, kv_ld};
+    CrossMma<T> pol{(const T*)q, (const T*)k, (const T*)v, bits, row_open, (T*)out, Lq, Lk, nh, hd, (Lk + 31) / 32, kv_ld, kv_bstride};
     return launch_flash<T>(pol, dm, hd, workspace, st, "cross_attention(mma)");
   }
   using T = __half;
-  CrossMma<T> pol{(const T*)q, (const T*)k, (const T*)v, bits, row_open, (T*)out, Lq, Lk, nh, hd, (Lk + 31) / 32, kv_ld};
+  CrossMma<T> pol{(const T*)q, (const T*)k, (const T*)v, bits, row_open, (T*)out, Lq, Lk, nh, hd, (Lk + 31) / 32, kv_ld, kv_bstride};
   return launch_flash<T>(pol, dm, hd, workspace, st, "cross_attention(mma)");
+}
+
+int mma_prefix_causal_attention(const void* qkv, const void* pk, const void* pv, int P, int ld_rows, const uint8_t* key_valid,
+                                void* out, int B, int T_, int nh, int hd, int dtype, cudaStream_t st) {
+  const int Pt = (P + 63) / 64;
+  AttnDims dm{B, nh, T_, Pt * 64 + T_, 1, 1.0f / sqrtf((float)hd)};
+  if (dtype == PSALM_BF16) {
+    using T = __nv_bfloat16;
+    PrefixCausalMma<T> pol{(const T*)qkv, (const T*)pk, (const T*)pv, key_valid, (T*)out, T_, nh, hd, P, ld_rows, Pt};
+    return launch_flash<T>(pol, dm, hd, nullptr, st, "prefix_causal_attention(mma)");
+  }
+  using T = __half;
+  PrefixCausalMma<T> pol{(const T*)qkv, (const T*)pk, (const T*)pv, key_valid, (T*)out, T_, nh, hd, P, ld_rows, Pt};
+  return launch_flash<T>(pol, dm, hd, nullptr, st, "prefix_causal_attention(mma)");
 }
 
 template <typename T>

@@ -114,6 +114,42 @@ struct CausalPolicy {
   }
 };
 
+// Causal prefill of prompt suffixes behind a shared prefix (key axis = [P prefix keys | own keys]): the prefix K / V are
+// head-major [nh, ld_rows, hd] and shared by all B sequences; query t attends the prefix and its own keys u <= t.
+template <typename T>
+struct PrefixCausalPolicy {
+  const T* qkv;              // [B, T, 3, nh, hd], rotary applied at positions P + t
+  const T *pk, *pv;          // [nh, ld_rows, hd]
+  const uint8_t* key_valid;  // [B, T] or null
+  T* out;                    // [B, T, nh*hd]
+  int T_, nh, hd, P, ld_rows;
+  __device__ __forceinline__ float4 load_q4(int b, int h, int n, int d0) const {
+    return ld4<T>(qkv + (((size_t)b * T_ + n) * 3) * nh * hd + h * hd + d0);
+  }
+  __device__ __forceinline__ float4 load_k4(int b, int h, int kj, int d0) const {
+    if (kj < P) return ld4<T>(pk + ((size_t)h * ld_rows + kj) * hd + d0);
+    return ld4<T>(qkv + (((size_t)b * T_ + kj - P) * 3 + 1) * nh * hd + h * hd + d0);
+  }
+  __device__ __forceinline__ float4 load_v4(int b, int h, int kj, int d0) const {
+    if (kj < P) return ld4<T>(pv + ((size_t)h * ld_rows + kj) * hd + d0);
+    return ld4<T>(qkv + (((size_t)b * T_ + kj - P) * 3 + 2) * nh * hd + h * hd + d0);
+  }
+  __device__ __forceinline__ float score(int b, int h, int qi, int kj, float s) const {
+    if (kj < P) return s;
+    const int u = kj - P;
+    if (u > qi) return -INFINITY;
+    if (key_valid && !key_valid[(size_t)b * T_ + u]) return -INFINITY;
+    return s;
+  }
+  __device__ __forceinline__ int key_tile_end(int q0, int kt1) const {
+    const int e = (P + q0 + kBQ - 1) / kBK + 1;
+    return e < kt1 ? e : kt1;
+  }
+  __device__ __forceinline__ void store(int b, int h, int n, int d, float v) const {
+    out[((size_t)b * T_ + n) * nh * hd + h * hd + d] = from_f32<T>(v);
+  }
+};
+
 template <typename T>
 struct CrossPolicy {
   const T *q, *k, *v;        // [B, Lq, nh*hd], [B, Lk, nh*hd] x2
@@ -359,7 +395,9 @@ namespace psalm {
 // tensor-core paths (attn_mma.cu)
 int mma_causal_attention(const void*, const uint8_t*, void*, int, int, int, int, int, cudaStream_t);
 int mma_cross_attention(const void*, const void*, const void*, const uint32_t*, const uint8_t*, void*, float*, int,
-                        int, int, int, int, int, int, cudaStream_t, int kv_ld = 0);
+                        int, int, int, int, int, int, cudaStream_t, int kv_ld = 0, long long kv_bstride = -1);
+int mma_prefix_causal_attention(const void*, const void*, const void*, int, int, const uint8_t*, void*, int, int, int, int,
+                                int, cudaStream_t);
 int mma_window_attention(const void*, const void*, const float*, void*, int, int, int, int, int, int, int,
                          cudaStream_t);
 extern int g_splitk_mode;
@@ -418,6 +456,30 @@ extern "C" int psalm_causal_attention(const void* qkv, const uint8_t* key_valid,
   DISPATCH_T(dtype, {
     CausalPolicy<T> pol{(const T*)qkv, key_valid, (T*)out, T_, nh, hd};
     rc = launch_attn(pol, dm, B, hd, nullptr, (cudaStream_t)stream, "causal_attention");
+  });
+  return rc;
+}
+
+extern "C" int psalm_prefix_causal_attention(const void* qkv, const void* prefix_k, const void* prefix_v, int P,
+                                             int prefix_ld_rows, const uint8_t* key_valid, void* out, int B, int T_, int nh,
+                                             int hd, int dtype, void* stream) {
+  PSALM_REQUIRE(qkv && out, "prefix_causal_attention: null pointer");
+  PSALM_REQUIRE(P >= 0 && prefix_ld_rows >= P && (P == 0 || (prefix_k && prefix_v)),
+                "prefix_causal_attention: bad prefix (P=%d, ld_rows=%d)", P, prefix_ld_rows);
+  PSALM_REQUIRE(B >= 1 && T_ >= 1 && nh >= 1 && hd % 4 == 0, "prefix_causal_attention: bad B / T / nh / hd");
+  if (dtype != PSALM_F32 && g_attn_impl == 0 && (hd == 32 || hd == 64)) {
+    PSALM_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)prefix_k & 15) == 0 && ((uintptr_t)prefix_v & 15) == 0,
+                  "prefix_causal_attention: pointers must be 16-byte aligned");
+    PSALM_REQUIRE((P + 63) / 64 * 64 + T_ <= 128 * 64, "prefix_causal_attention: padded prefix + T must be <= 8192 keys");
+    return mma_prefix_causal_attention(qkv, prefix_k, prefix_v, P, prefix_ld_rows, key_valid, out, B, T_, nh, hd, dtype,
+                                       (cudaStream_t)stream);
+  }
+  AttnDims dm{B, nh, T_, P + T_, 1, 1.0f / sqrtf((float)hd)};
+  int rc = PSALM_OK;
+  DISPATCH_T(dtype, {
+    PrefixCausalPolicy<T> pol{(const T*)qkv, (const T*)prefix_k, (const T*)prefix_v, key_valid, (T*)out, T_, nh, hd, P,
+                              prefix_ld_rows};
+    rc = launch_attn(pol, dm, B, hd, nullptr, (cudaStream_t)stream, "prefix_causal_attention");
   });
   return rc;
 }

@@ -16,7 +16,7 @@ namespace psalm {
 // SIMT fp32 tile kernel: CTA = 32 queries x 128 pixels, K chunks of 32; thread = 2 q x 8 p.
 template <typename T, typename TO>
 __global__ void __launch_bounds__(256) mask_logits_kernel(const T* __restrict__ A, const T* __restrict__ F,
-                                                          TO* __restrict__ out, int Q, int P, int C) {
+                                                          TO* __restrict__ out, int Q, int P, int C, long long fbs) {
   constexpr int TQ = 32, TP = 128, TK = 32;
   __shared__ float As[TK][TQ + 1];
   __shared__ float Fs[TK][TP + 1];
@@ -30,7 +30,7 @@ __global__ void __launch_bounds__(256) mask_logits_kernel(const T* __restrict__ 
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
   const T* Ab = A + (size_t)b * Q * C;
-  const T* Fb = F + (size_t)b * P * C;
+  const T* Fb = F + (size_t)b * fbs;   // fbs = P * C, or 0: one feature map for every query set
   for (int k0 = 0; k0 < C; k0 += TK) {
     for (int i = tid; i < TQ * TK; i += 256) {
       const int qq = i / TK, kk = i % TK;
@@ -154,8 +154,8 @@ __global__ void attn_mask_bits_kernel(const T* __restrict__ logits, uint32_t* __
 }  // namespace psalm
 
 namespace psalm {
-int mma_mask_proj(const void* me, const void* feats, void* out, uint32_t* bits, uint8_t* row_open, int B, int Q, int P,
-                  int dtype, cudaStream_t st);
+int mma_mask_proj(const void* me, const void* feats, long long feats_bstride, void* out, uint32_t* bits, uint8_t* row_open,
+                  int B, int Q, int P, int dtype, cudaStream_t st);
 static int g_mask_proj_impl = 0;   // 0 auto, 1 mma.sync, 2 wgmma GEMM where it applies
 }
 
@@ -169,35 +169,53 @@ extern "C" int psalm_set_mask_proj_impl(int impl) {
 
 extern "C" int psalm_mask_bits_fused(const void* mask_embed, const void* feats, uint32_t* bits, uint8_t* row_open,
                                      int B, int Q, int P, int C, int dtype, void* stream) {
+  return psalm_mask_bits_fused_strided(mask_embed, feats, (long long)P * C, bits, row_open, B, Q, P, C, dtype, stream);
+}
+
+extern "C" int psalm_mask_bits_fused_strided(const void* mask_embed, const void* feats, long long feats_batch_stride,
+                                             uint32_t* bits, uint8_t* row_open, int B, int Q, int P, int C, int dtype,
+                                             void* stream) {
   PSALM_REQUIRE(mask_embed && feats && bits && row_open, "mask_bits_fused: null pointer");
+  PSALM_REQUIRE(feats_batch_stride >= 0 && feats_batch_stride % 8 == 0,
+                "mask_bits_fused: feature batch stride %lld must be >= 0 and a multiple of 8", feats_batch_stride);
   if (dtype == PSALM_F32 || C != 256 || Q > 112) {
     set_error("mask_bits_fused: needs 16-bit storage, C == 256, Q <= 112 (got dtype %d, C %d, Q %d)", dtype, C, Q);
     return PSALM_E_UNSUPPORTED;
   }
-  return mma_mask_proj(mask_embed, feats, nullptr, bits, row_open, B, Q, P, dtype, (cudaStream_t)stream);
+  return mma_mask_proj(mask_embed, feats, feats_batch_stride, nullptr, bits, row_open, B, Q, P, dtype, (cudaStream_t)stream);
 }
 
 extern "C" int psalm_mask_logits(const void* mask_embed, const void* feats, void* out, int B, int Q, int P,
                                  int C, int dtype, int out_dtype, void* stream) {
+  return psalm_mask_logits_strided(mask_embed, feats, (long long)P * C, out, B, Q, P, C, dtype, out_dtype, stream);
+}
+
+extern "C" int psalm_mask_logits_strided(const void* mask_embed, const void* feats, long long feats_batch_stride, void* out,
+                                         int B, int Q, int P, int C, int dtype, int out_dtype, void* stream) {
   PSALM_REQUIRE(mask_embed && feats && out, "mask_logits: null pointer");
   PSALM_REQUIRE(out_dtype == dtype || out_dtype == PSALM_F32, "mask_logits: out dtype must be F32 or the input dtype");
-  // large maps: per image one wgmma GEMM out[b] = mask_embed[b] (Q x C, TMA zero-fills rows Q..127 of the tile) ·
-  // feats[b]ᵀ (P x C), both operands K-major as stored (csrc/gemm_wgmma.cu)
+  PSALM_REQUIRE(feats_batch_stride >= 0, "mask_logits: negative feature batch stride %lld", feats_batch_stride);
+  // large maps: wgmma GEMMs out[b] = mask_embed[b] (Q x C, TMA zero-fills rows Q..127 of the tile) · feats[b]ᵀ (P x C),
+  // both operands K-major as stored (csrc/gemm_wgmma.cu): one per image, or ONE with M = B * Q rows when every query set
+  // reads the same feature map (stride 0: mask_embed [B, Q, C] is already [B * Q, C], out [B, Q, P] is [B * Q, P])
   if (dtype != PSALM_F32 && out_dtype == dtype && C == 256 && Q <= 128 && P % 256 == 0 &&
       (g_mask_proj_impl == 2 || (g_mask_proj_impl == 0 && P >= 8192))) {
+    if (feats_batch_stride == 0)
+      return psalm_linear_fused(mask_embed, C, feats, nullptr, out, (long long)B * Q, P, C, 0, 0, dtype, stream);
     const size_t es = dtype_size(dtype);
     for (int b = 0; b < B; ++b) {
-      const int rc = psalm_linear_fused((const char*)mask_embed + (size_t)b * Q * C * es, C, (const char*)feats + (size_t)b * P * C * es,
-                                        nullptr, (char*)out + (size_t)b * Q * P * es, Q, P, C, 0, 0, dtype, stream);
+      const int rc = psalm_linear_fused((const char*)mask_embed + (size_t)b * Q * C * es, C,
+                                        (const char*)feats + (size_t)b * feats_batch_stride * es, nullptr,
+                                        (char*)out + (size_t)b * Q * P * es, Q, P, C, 0, 0, dtype, stream);
       if (rc != PSALM_OK) return rc;
     }
     return PSALM_OK;
   }
-  if (dtype != PSALM_F32 && out_dtype == dtype && C == 256 && Q <= 112 && P % 2 == 0)
-    return mma_mask_proj(mask_embed, feats, out, nullptr, nullptr, B, Q, P, dtype, (cudaStream_t)stream);
+  if (dtype != PSALM_F32 && out_dtype == dtype && C == 256 && Q <= 112 && P % 2 == 0 && feats_batch_stride % 8 == 0)
+    return mma_mask_proj(mask_embed, feats, feats_batch_stride, out, nullptr, nullptr, B, Q, P, dtype, (cudaStream_t)stream);
   dim3 grid((P + 127) / 128, (Q + 31) / 32, B);
   cudaStream_t st = (cudaStream_t)stream;
-#define ML(T, TO) mask_logits_kernel<T, TO><<<grid, 256, 0, st>>>((const T*)mask_embed, (const T*)feats, (TO*)out, Q, P, C)
+#define ML(T, TO) mask_logits_kernel<T, TO><<<grid, 256, 0, st>>>((const T*)mask_embed, (const T*)feats, (TO*)out, Q, P, C, feats_batch_stride)
   if (dtype == PSALM_F32) ML(float, float);
   else if (dtype == PSALM_F16) { if (out_dtype == PSALM_F32) ML(__half, float); else ML(__half, __half); }
   else if (dtype == PSALM_BF16) { if (out_dtype == PSALM_F32) ML(__nv_bfloat16, float); else ML(__nv_bfloat16, __nv_bfloat16); }

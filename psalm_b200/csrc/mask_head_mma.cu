@@ -40,14 +40,14 @@ __device__ __forceinline__ void mh_mma(float (&d)[4], const uint32_t (&a)[4], ui
 template <typename T, int TP, bool kBits>
 __global__ void __launch_bounds__(128) mask_proj_mma_kernel(const T* __restrict__ me, const T* __restrict__ feats,
                                                             T* __restrict__ out, uint32_t* __restrict__ bits,
-                                                            int Q, int P, int W32) {
+                                                            int Q, int P, int W32, long long fbs) {
   extern __shared__ __align__(16) unsigned char mh_smem[];
   T* As = reinterpret_cast<T*>(mh_smem);          // [MH_QP][MH_LD]  mask_embed
   T* Bs = As + MH_QP * MH_LD;                     // [TP][MH_LD]     feats tile
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.y, p0 = blockIdx.x * TP;
   const T* meb = me + (size_t)b * Q * MH_C;
-  const T* fb = feats + (size_t)b * P * MH_C;
+  const T* fb = feats + (size_t)b * fbs;   // fbs = P * C, or 0: one feature map for every query set
   for (int i = tid; i < MH_QP * (MH_C / 8); i += 128) {
     const int row = i / (MH_C / 8), c8 = (i % (MH_C / 8)) * 8;
     const bool ok = row < Q;
@@ -147,7 +147,7 @@ __global__ void row_open_kernel(const uint32_t* __restrict__ bits, uint8_t* __re
 
 template <typename T>
 static int launch_mask_proj(const void* me, const void* feats, void* out, uint32_t* bits, uint8_t* row_open, int B,
-                            int Q, int P, cudaStream_t st) {
+                            int Q, int P, long long fbs, cudaStream_t st) {
   const int W32 = (P + 31) / 32;
   cudaError_t e;
   if (bits) {
@@ -156,7 +156,7 @@ static int launch_mask_proj(const void* me, const void* feats, void* out, uint32
     e = cudaFuncSetAttribute(mask_proj_mma_kernel<T, TP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("mask_proj: %s", cudaGetErrorString(e)); return PSALM_E_CUDA; }
     dim3 grid((P + TP - 1) / TP, B);
-    mask_proj_mma_kernel<T, TP, true><<<grid, 128, smem, st>>>((const T*)me, (const T*)feats, nullptr, bits, Q, P, W32);
+    mask_proj_mma_kernel<T, TP, true><<<grid, 128, smem, st>>>((const T*)me, (const T*)feats, nullptr, bits, Q, P, W32, fbs);
     row_open_kernel<<<(B * Q * 32 + 255) / 256, 256, 0, st>>>(bits, row_open, B * Q, P, W32);
   } else {
     constexpr int TP = 64;
@@ -164,15 +164,15 @@ static int launch_mask_proj(const void* me, const void* feats, void* out, uint32
     e = cudaFuncSetAttribute(mask_proj_mma_kernel<T, TP, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("mask_proj: %s", cudaGetErrorString(e)); return PSALM_E_CUDA; }
     dim3 grid((P + TP - 1) / TP, B);
-    mask_proj_mma_kernel<T, TP, false><<<grid, 128, smem, st>>>((const T*)me, (const T*)feats, (T*)out, nullptr, Q, P, W32);
+    mask_proj_mma_kernel<T, TP, false><<<grid, 128, smem, st>>>((const T*)me, (const T*)feats, (T*)out, nullptr, Q, P, W32, fbs);
   }
   return check_launch("mask_proj_mma_kernel");
 }
 
-int mma_mask_proj(const void* me, const void* feats, void* out, uint32_t* bits, uint8_t* row_open, int B, int Q, int P,
-                  int dtype, cudaStream_t st) {
-  if (dtype == PSALM_BF16) return launch_mask_proj<__nv_bfloat16>(me, feats, out, bits, row_open, B, Q, P, st);
-  return launch_mask_proj<__half>(me, feats, out, bits, row_open, B, Q, P, st);
+int mma_mask_proj(const void* me, const void* feats, long long feats_bstride, void* out, uint32_t* bits, uint8_t* row_open,
+                  int B, int Q, int P, int dtype, cudaStream_t st) {
+  if (dtype == PSALM_BF16) return launch_mask_proj<__nv_bfloat16>(me, feats, out, bits, row_open, B, Q, P, feats_bstride, st);
+  return launch_mask_proj<__half>(me, feats, out, bits, row_open, B, Q, P, feats_bstride, st);
 }
 
 }  // namespace psalm

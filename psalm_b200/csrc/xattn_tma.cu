@@ -61,6 +61,7 @@ struct XaParams {
   float* part_o;             // [B, splits, 8, 112, 32]
   float* part_ml;            // [B, splits, 8, 112, 2]
   int B, Lq, Lk, W32, splits, steps_per_split;
+  int kv_batch_rows;         // K / V rows between consecutive images in the tensor maps: Lk, or 0 = one shared memory
   float qscale;              // 1/sqrt(hd) * log2(e)
 };
 
@@ -310,7 +311,7 @@ xattn_tma_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
       if (it >= STAGES) mbar_wait(&empty[stage], ((it / STAGES) - 1) & 1);   // all 8 warps are done with the old tile
       mbar_arrive_expect_tx(&full[stage], (uint32_t)STAGE_BYTES);
       unsigned char* dst = kv + (size_t)stage * STAGE_BYTES;
-      const int row0 = b * p.Lk + (step0 + it) * KS;
+      const int row0 = b * p.kv_batch_rows + (step0 + it) * KS;
 #pragma unroll
       for (int bx = 0; bx < HPC / 2; ++bx) {
         tma_load_2d(dst + bx * BOX_BYTES, &mapK, (hg * (HPC / 2) + bx) * 64, row0, &full[stage]);
@@ -518,7 +519,7 @@ static int xa_splits(int B, int Lk) {
 static int g_cross_impl = 0;   // 0 auto, 1 / 2 always the TMA-fed kernel of this file
 // per-head flash kernel of attn_mma.cu (row-strided K / V views supported)
 int mma_cross_attention(const void*, const void*, const void*, const uint32_t*, const uint8_t*, void*, float*, int, int, int, int,
-                        int, int, int, cudaStream_t, int kv_ld);
+                        int, int, int, cudaStream_t, int kv_ld, long long kv_bstride);
 constexpr int kSmallLk = 2048;   // below this many keys the problem is launch / latency bound: the per-head kernel with
                                  // few key tiles per CTA wins (measured, tools/bench_cross.py)
 static int small_splits(int B, int Lk) {
@@ -554,6 +555,15 @@ extern "C" int psalm_masked_cross_attention(const void* q, const void* k, const 
                                             const uint32_t* mask_bits, const uint8_t* row_open, void* out,
                                             float* workspace, size_t workspace_bytes, int B, int Lq, int Lk, int nh,
                                             int hd, int dtype, void* stream) {
+  return psalm_masked_cross_attention_strided(q, k, v, kv_row_stride, (long long)Lk * kv_row_stride, mask_bits, row_open, out,
+                                              workspace, workspace_bytes, B, Lq, Lk, nh, hd, dtype, stream);
+}
+
+extern "C" int psalm_masked_cross_attention_strided(const void* q, const void* k, const void* v, long long kv_row_stride,
+                                                    long long kv_batch_stride, const uint32_t* mask_bits,
+                                                    const uint8_t* row_open, void* out, float* workspace,
+                                                    size_t workspace_bytes, int B, int Lq, int Lk, int nh, int hd, int dtype,
+                                                    void* stream) {
   using namespace psalm;
   PSALM_REQUIRE(q && k && v && out, "masked_cross_attention: null pointer");
   PSALM_REQUIRE(nh == xa::NH && hd == xa::HD, "masked_cross_attention: needs 8 heads x 32 (got %d x %d)", nh, hd);
@@ -561,16 +571,23 @@ extern "C" int psalm_masked_cross_attention(const void* q, const void* k, const 
   PSALM_REQUIRE(Lq >= 1 && Lq <= xa::ROWS, "masked_cross_attention: 1..%d queries (got %d)", xa::ROWS, Lq);
   PSALM_REQUIRE(B >= 1 && B <= 65535 && Lk >= 1, "masked_cross_attention: bad B / Lk");
   PSALM_REQUIRE(kv_row_stride >= xa::C && kv_row_stride % 8 == 0, "masked_cross_attention: K/V row stride %lld", kv_row_stride);
+  PSALM_REQUIRE(kv_batch_stride >= 0 && kv_batch_stride % kv_row_stride == 0 &&
+                    (long long)(B - 1) * (kv_batch_stride / kv_row_stride) + Lk < (1ll << 31),
+                "masked_cross_attention: K/V batch stride %lld must be 0 or a multiple of the row stride %lld", kv_batch_stride,
+                kv_row_stride);
   PSALM_REQUIRE(((uintptr_t)k & 15) == 0 && ((uintptr_t)v & 15) == 0 && ((uintptr_t)q & 15) == 0 && ((uintptr_t)out & 3) == 0,
                 "masked_cross_attention: pointers must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   if (g_cross_impl == 0 && Lk < kSmallLk) {
     const int ss = small_splits(B, Lk);
-    return mma_cross_attention(q, k, v, mask_bits, row_open, out, workspace, B, Lq, Lk, nh, hd, ss, dtype, st, (int)kv_row_stride);
+    return mma_cross_attention(q, k, v, mask_bits, row_open, out, workspace, B, Lq, Lk, nh, hd, ss, dtype, st, (int)kv_row_stride,
+                               kv_batch_stride);
   }
+  const long long batch_rows = kv_batch_stride / kv_row_stride;
   XaParams p;
   p.q = q; p.bits = mask_bits; p.row_open = row_open; p.out = out;
   p.B = B; p.Lq = Lq; p.Lk = Lk; p.W32 = (Lk + 31) / 32;
+  p.kv_batch_rows = (int)batch_rows;
   p.splits = xa_splits(B, Lk);
   const int steps = (Lk + xa::KS - 1) / xa::KS;
   p.steps_per_split = (steps + p.splits - 1) / p.splits;
@@ -583,7 +600,8 @@ extern "C" int psalm_masked_cross_attention(const void* q, const void* k, const 
     p.part_ml = workspace + (size_t)B * p.splits * xa::NH * xa::ROWS * xa::HD;
   }
   CUtensorMap mk, mv;
-  if (!make_kv_map(&mk, k, (long long)B * Lk, kv_row_stride, dtype) || !make_kv_map(&mv, v, (long long)B * Lk, kv_row_stride, dtype)) {
+  const long long map_rows = (long long)(B - 1) * batch_rows + Lk;
+  if (!make_kv_map(&mk, k, map_rows, kv_row_stride, dtype) || !make_kv_map(&mv, v, map_rows, kv_row_stride, dtype)) {
     set_error("masked_cross_attention: cuTensorMapEncodeTiled failed (driver without TMA support?)");
     return PSALM_E_CUDA;
   }

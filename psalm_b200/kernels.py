@@ -102,6 +102,39 @@ def causal_attention(qkv, key_valid, B, T, nh, hd):
     return out
 
 
+@_on_device
+def prefix_causal_attention(qkv, prefix_k, prefix_v, P, key_valid, B, T, nh, hd):
+    """qkv [B,T,3,nh,hd] (rotary applied at positions P + t) behind a shared prefix whose K / V rows are prefix_k /
+    prefix_v [nh, ld_rows, hd] (rows 0..P-1 used) -> [B,T,nh*hd]; key_valid uint8 [B,T] or None."""
+    _chk(qkv, "prefix_causal_attention.qkv")
+    for t, n in ((prefix_k, "prefix_k"), (prefix_v, "prefix_v")):
+        _chk(t, "prefix_causal_attention." + n)
+        if t.dtype != qkv.dtype or t.dim() != 3 or t.shape[0] != nh or t.shape[2] != hd or t.shape[1] < P:
+            raise _lib.PsalmKernelError("prefix_causal_attention.%s: expected [%d, >= %d, %d] of %s" % (n, nh, P, hd, qkv.dtype))
+    if key_valid is not None:
+        _chk(key_valid, "prefix_causal_attention.key_valid")
+        if key_valid.dtype != torch.uint8 or tuple(key_valid.shape) != (B, T):
+            raise _lib.PsalmKernelError("prefix_causal_attention: key_valid must be uint8 [B,T]")
+    out = torch.empty((B, T, nh * hd), dtype=qkv.dtype, device=qkv.device)
+    rc = _lib.lib().psalm_prefix_causal_attention(_lib.ptr(qkv), _lib.ptr(prefix_k), _lib.ptr(prefix_v), int(P),
+                                                  prefix_k.shape[1], _lib.ptr(key_valid) if key_valid is not None else None,
+                                                  _lib.ptr(out), B, T, nh, hd, _lib.dtype_code(qkv.dtype),
+                                                  _lib.stream_ptr(qkv.device))
+    _lib.check(rc, "psalm_prefix_causal_attention")
+    _count()
+    return out
+
+
+def _batch_stride(t, dense, name):
+    """Batch stride of a [B, N, C] operand: `dense` (the usual layout) or 0 for an `expand`ed view of one image's map."""
+    if t.shape[0] == 1 or t.stride(0) == dense:
+        return dense
+    if t.stride(0) == 0:
+        return 0
+    raise _lib.PsalmKernelError("%s: batch stride must be %d or 0 (an expand view of one image), got %d"
+                                % (name, dense, t.stride(0)))
+
+
 def pick_splits(B, nh, Lq, Lk):
     """Split-K factor so that a 100-query problem still fills ~2 waves of 132 SMs."""
     ctas = B * nh * ((Lq + 63) // 64)
@@ -138,16 +171,23 @@ def cross_attention(q, k, v, mask_bits=None, row_open=None, nh=8, splits=None, w
 
 @_on_device
 def mask_logits(mask_embed, feats, out_dtype=None):
-    """mask_embed [B,Q,C], feats [B,P,C] (token-major) -> [B,Q,P]."""
+    """mask_embed [B,Q,C], feats [B,P,C] (token-major) -> [B,Q,P].  feats may be a stride-0 `expand(B, P, C)` view of
+    one image's map: every query set then reads that map (the prompts of one image)."""
     _chk(mask_embed, "mask_logits.mask_embed")
-    _chk(feats, "mask_logits.feats")
+    _chk(feats[0], "mask_logits.feats")
     B, Q, C = mask_embed.shape
     P = feats.shape[1]
+    fbs = _batch_stride(feats, P * C, "mask_logits.feats")
     out_dtype = out_dtype or mask_embed.dtype
     out = torch.empty((B, Q, P), dtype=out_dtype, device=feats.device)
-    rc = _lib.lib().psalm_mask_logits(_lib.ptr(mask_embed), _lib.ptr(feats), _lib.ptr(out), B, Q, P, C,
-                                      _lib.dtype_code(feats.dtype), _lib.dtype_code(out_dtype),
-                                      _lib.stream_ptr(feats.device))
+    if fbs == P * C:
+        rc = _lib.lib().psalm_mask_logits(_lib.ptr(mask_embed), _lib.ptr(feats), _lib.ptr(out), B, Q, P, C,
+                                          _lib.dtype_code(feats.dtype), _lib.dtype_code(out_dtype),
+                                          _lib.stream_ptr(feats.device))
+    else:
+        rc = _lib.lib().psalm_mask_logits_strided(_lib.ptr(mask_embed), _lib.ptr(feats), fbs, _lib.ptr(out), B, Q, P, C,
+                                                  _lib.dtype_code(feats.dtype), _lib.dtype_code(out_dtype),
+                                                  _lib.stream_ptr(feats.device))
     _lib.check(rc, "psalm_mask_logits")
     _count()
     return out
@@ -289,15 +329,21 @@ def mask_bits(mask_embed, feats):
     (bits int32 [B,Q,ceil(P/32)], row_open uint8 [B,Q]).  16-bit storage: one tensor-core kernel that never
     writes the logits; fp32 storage: exact fp32 projection + threshold kernel."""
     _chk(mask_embed, "mask_bits.mask_embed")
-    _chk(feats, "mask_bits.feats")
+    _chk(feats[0], "mask_bits.feats")
     B, Q, C = mask_embed.shape
     P = feats.shape[1]
+    fbs = _batch_stride(feats, P * C, "mask_bits.feats")   # 0: stride-0 expand view of one image's map
     if mask_embed.dtype == torch.float32 or C != 256 or Q > 112:
         return attn_mask_bits(mask_logits(mask_embed, feats, out_dtype=torch.float32))
     bits = torch.empty((B, Q, (P + 31) // 32), dtype=torch.int32, device=feats.device)
     row_open = torch.empty((B, Q), dtype=torch.uint8, device=feats.device)
-    rc = _lib.lib().psalm_mask_bits_fused(_lib.ptr(mask_embed), _lib.ptr(feats), _lib.ptr(bits), _lib.ptr(row_open),
-                                          B, Q, P, C, _lib.dtype_code(feats.dtype), _lib.stream_ptr(feats.device))
+    if fbs == P * C:
+        rc = _lib.lib().psalm_mask_bits_fused(_lib.ptr(mask_embed), _lib.ptr(feats), _lib.ptr(bits), _lib.ptr(row_open),
+                                              B, Q, P, C, _lib.dtype_code(feats.dtype), _lib.stream_ptr(feats.device))
+    else:
+        rc = _lib.lib().psalm_mask_bits_fused_strided(_lib.ptr(mask_embed), _lib.ptr(feats), fbs, _lib.ptr(bits),
+                                                      _lib.ptr(row_open), B, Q, P, C, _lib.dtype_code(feats.dtype),
+                                                      _lib.stream_ptr(feats.device))
     _lib.check(rc, "psalm_mask_bits_fused")
     _count(2)
     return bits, row_open
@@ -414,27 +460,31 @@ def patchify(images, out_dtype, mean=None, std=None, patch=4):
 
 @_on_device
 def masked_cross_attention(q, k, v, mask_bits=None, row_open=None, nh=8, workspace=None):
-    """q [B,Lq,256]; k, v [B,Lk,256] possibly ROW-STRIDED views (last dim contiguous, batch stride = Lk * row stride)
-    -> [B,Lq,256].  TMA-fed kernel of csrc/xattn_tma.cu (16-bit storage, 8 heads x 32)."""
+    """q [B,Lq,256]; k, v [B,Lk,256] possibly ROW-STRIDED views (last dim contiguous, batch stride = Lk * row stride,
+    or 0 for `expand`ed views of one image's memory shared by the B query sets) -> [B,Lq,256].  TMA-fed kernel of
+    csrc/xattn_tma.cu (16-bit storage, 8 heads x 32)."""
     _chk(q, "masked_cross_attention.q")
     B, Lq, C = q.shape
     Lk = k.shape[1]
     ld = k.stride(1)
+    bstride = Lk * ld if B == 1 else k.stride(0)
     for t, n in ((k, "k"), (v, "v")):
         if not t.is_cuda or t.dtype != q.dtype or tuple(t.shape) != (B, Lk, C) or t.stride(2) != 1 or t.stride(1) != ld or \
-                (B > 1 and t.stride(0) != Lk * ld):
-            raise _lib.PsalmKernelError("masked_cross_attention.%s: expected a [B,Lk,%d] view with contiguous rows and a "
-                                        "common row stride" % (n, C))
+                (B > 1 and (t.stride(0) != bstride or bstride not in (0, Lk * ld))):
+            raise _lib.PsalmKernelError("masked_cross_attention.%s: expected a [B,Lk,%d] view with contiguous rows, a "
+                                        "common row stride and a batch stride of Lk rows or 0" % (n, C))
     L = _lib.lib()
     need = L.psalm_masked_cross_attention_workspace_bytes(B, Lq, Lk)
     if need and (workspace is None or workspace.numel() * workspace.element_size() < need):
         workspace = torch.empty(need // 4, dtype=torch.float32, device=q.device)
     out = torch.empty_like(q)
-    rc = L.psalm_masked_cross_attention(
-        _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), ld, _lib.ptr(mask_bits) if mask_bits is not None else None,
-        _lib.ptr(row_open) if row_open is not None else None, _lib.ptr(out),
-        _lib.ptr(workspace) if need else None, workspace.numel() * workspace.element_size() if need else 0,
-        B, Lq, Lk, nh, C // nh, _lib.dtype_code(q.dtype), _lib.stream_ptr(q.device))
+    args = (_lib.ptr(mask_bits) if mask_bits is not None else None, _lib.ptr(row_open) if row_open is not None else None,
+            _lib.ptr(out), _lib.ptr(workspace) if need else None, workspace.numel() * workspace.element_size() if need else 0,
+            B, Lq, Lk, nh, C // nh, _lib.dtype_code(q.dtype), _lib.stream_ptr(q.device))
+    if bstride == Lk * ld:
+        rc = L.psalm_masked_cross_attention(_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), ld, *args)
+    else:
+        rc = L.psalm_masked_cross_attention_strided(_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), ld, 0, *args)
     _lib.check(rc, "psalm_masked_cross_attention")
     _count(2 if need else 1)
     return out

@@ -87,22 +87,23 @@ class MultiScaleMaskedTransformerDecoderForOPTPreTrain:
         out["aux_outputs"] = []
         return out
 
-    def forward_tokens(self, ms_tokens, ms_sizes, mask_features, mf_size, seg_query, SEG_embedding=None,
-                       class_name_embedding=None, return_trace=False, hooks=None, region_embedding_list=None):
-        """ms_tokens: 3 maps [B,HW_l,256] (32^2,64^2,128^2 levels); mask_features [B,H4*W4,256];
-        seg_query [B,Q,256].  Returns dict(pred_masks [B,Q,H4*W4], pred_class_name_logits, pred_SEG_logits).
-        `hooks` (tests only, oracle/parity.py): an object whose before_layer(i, output, bits, row_open, mask_for) may
-        substitute the decoder state / attention mask entering layer i (layer-wise teacher forcing) and whose
-        after_layer(i, output) observes the state leaving it."""
-        cfg, w = self.cfg, self.w
-        B, Q, Hd = seg_query.shape
-        nh = cfg.nheads
-        H4, W4 = mf_size
+    def _fused_kv(self, Q, Hd):
         # 16-bit storage: all K / V projections of a level up front (one GEMM each), consumed as row-strided views by
         # the TMA-fed kernel; fp32 storage keeps the per-layer projections + the SIMT kernel
-        fused_kv = self.dtype != torch.float32 and Hd == 256 and nh == 8 and Q <= 112
+        return self.dtype != torch.float32 and Hd == 256 and self.cfg.nheads == 8 and Q <= 112
+
+    def memory(self, ms_tokens, ms_sizes, mask_features, mf_size, Q=None):
+        """The query-independent part of forward_tokens for images [B]: the K / V projections of the three levels (16-bit
+        storage) or their inputs (fp32), and mask_features pooled to the three attention-mask sizes.  A memory of ONE
+        image serves any number of query sets (forward_tokens(..., memory=...), the prompts of one image)."""
+        cfg, w = self.cfg, self.w
+        Hd = ms_tokens[0].shape[-1]
+        Q = cfg.num_queries if Q is None else Q
+        B = ms_tokens[0].shape[0]
+        H4, W4 = mf_size
+        mem = dict(B=B, fused_kv=self._fused_kv(Q, Hd), mask_features=mask_features)
         srcs, kins = [], []
-        if not fused_kv:
+        if not mem["fused_kv"]:
             for i in range(3):  # (:607-614); input_proj is the identity (in_channels == hidden_dim, :475-479)
                 Hl, Wl = ms_sizes[i]
                 pos = position_embedding_sine_tokens(Hl, Wl, self.device).to(self.dtype)
@@ -110,18 +111,9 @@ class MultiScaleMaskedTransformerDecoderForOPTPreTrain:
                 srcs.append(src)
                 kins.append(src + pos)
         # attention-mask sources: mask_features interpolated once to each target size (see module docstring)
-        pooled = [kernels.bilinear_tokens(mask_features, H4, W4, hl, wl) for hl, wl in ms_sizes]
-        qpos = self.query_embed.unsqueeze(0)
-        output = seg_query.to(self.dtype).contiguous()
-        trace = []
-
-        def mask_for(level, out_):
-            _, me = self._heads_common(out_)
-            if return_trace:
-                trace.append(kernels.mask_logits(me.contiguous(), pooled[level], out_dtype=torch.float32))
-            return kernels.mask_bits(me.contiguous(), pooled[level])
-
-        if fused_kv:
+        mem["pooled"] = [kernels.bilinear_tokens(mask_features, H4, W4, hl, wl) for hl, wl in ms_sizes]
+        mem["srcs"], mem["kins"] = srcs, kins
+        if mem["fused_kv"]:
             # K = (x + level_embed + pos) Wk^T + bk = x Wk^T + [(level_embed + pos) Wk^T + bk] and
             # V = (x + level_embed) Wv^T + bv = x Wv^T + [Wv level_embed + bv]: the bracketed terms do not depend on the
             # input, so they are projected once per (sizes, batch) and enter the GEMMs as the additive C matrix / the bias;
@@ -142,9 +134,54 @@ class MultiScaleMaskedTransformerDecoderForOPTPreTrain:
                               .to(self.dtype).contiguous())
                 kvc = self._kv_const[ckey] = (posk, vb)
             posk, vb = kvc
-            k_all = [torch.addmm(posk[li], ms_tokens[li].reshape(-1, Hd), w["xk_all%d.w" % li].t()).view(B, -1, 3 * Hd)
-                     for li in range(3)]
-            v_all = [F.linear(ms_tokens[li], w["xv_all%d.w" % li], vb[li]) for li in range(3)]
+            mem["k_all"] = [torch.addmm(posk[li], ms_tokens[li].reshape(-1, Hd), w["xk_all%d.w" % li].t()).view(B, -1, 3 * Hd)
+                            for li in range(3)]
+            mem["v_all"] = [F.linear(ms_tokens[li], w["xv_all%d.w" % li], vb[li]) for li in range(3)]
+        return mem
+
+    def forward_tokens(self, ms_tokens, ms_sizes, mask_features, mf_size, seg_query, SEG_embedding=None,
+                       class_name_embedding=None, return_trace=False, hooks=None, region_embedding_list=None, memory=None):
+        """ms_tokens: 3 maps [B,HW_l,256] (32^2,64^2,128^2 levels); mask_features [B,H4*W4,256];
+        seg_query [B,Q,256].  Returns dict(pred_masks [B,Q,H4*W4], pred_class_name_logits, pred_SEG_logits).
+        `memory`: the result of `memory(...)` for these maps (ms_tokens / mask_features are then not read); a memory of
+        one image with B query sets runs the B sets against that image.
+        `hooks` (tests only, oracle/parity.py): an object whose before_layer(i, output, bits, row_open, mask_for) may
+        substitute the decoder state / attention mask entering layer i (layer-wise teacher forcing) and whose
+        after_layer(i, output) observes the state leaving it."""
+        cfg, w = self.cfg, self.w
+        B, Q, Hd = seg_query.shape
+        nh = cfg.nheads
+        if memory is None:
+            memory = self.memory(ms_tokens, ms_sizes, mask_features, mf_size, Q)
+        fused_kv = memory["fused_kv"]
+        if fused_kv != self._fused_kv(Q, Hd):
+            raise ValueError("memory was prepared for another query shape")
+        shared = memory["B"] != B
+        if shared and memory["B"] != 1:
+            raise ValueError("a memory of %d images cannot serve %d query sets" % (memory["B"], B))
+
+        def per_set(t):
+            # one image's memory for B query sets: 16-bit kernels read stride-0 `expand` views; the fp32 parity path
+            # materialises copies where its kernels need dense batches (psalm_cross_attention has no batch stride)
+            if not shared:
+                return t
+            return t.expand(B, *t.shape[1:]) if fused_kv else t.expand(B, *t.shape[1:]).contiguous()
+
+        pooled = [per_set(t) for t in memory["pooled"]]
+        mask_features = per_set(memory["mask_features"])
+        srcs, kins = memory["srcs"], memory["kins"]
+        if fused_kv:
+            k_all, v_all = [per_set(t) for t in memory["k_all"]], [per_set(t) for t in memory["v_all"]]
+        qpos = self.query_embed.unsqueeze(0)
+        output = seg_query.to(self.dtype).contiguous()
+        trace = []
+
+        def mask_for(level, out_):
+            _, me = self._heads_common(out_)
+            if return_trace:
+                trace.append(kernels.mask_logits(me.contiguous(), pooled[level], out_dtype=torch.float32))
+            return kernels.mask_bits(me.contiguous(), pooled[level])
+
         qc = None
         fold_q = fused_kv and not os.environ.get("PSALM_NO_QCONST")
         if fold_q:
@@ -182,8 +219,8 @@ class MultiScaleMaskedTransformerDecoderForOPTPreTrain:
                 a = kernels.timed("masked_cross_attention_%d" % k.shape[1], kernels.masked_cross_attention, q, k, v,
                                   bits, row_open, nh)
             else:
-                k = F.linear(kins[li], w["x%d.k.w" % i], w["x%d.k.b" % i])
-                v = F.linear(srcs[li], w["x%d.v.w" % i], w["x%d.v.b" % i])
+                k = per_set(F.linear(kins[li], w["x%d.k.w" % i], w["x%d.k.b" % i]))
+                v = per_set(F.linear(srcs[li], w["x%d.v.w" % i], w["x%d.v.b" % i]))
                 a = kernels.timed("masked_cross_attention_%d" % k.shape[1], kernels.cross_attention, q, k, v, bits,
                                   row_open, nh)
             output = kernels.add_layer_norm(output, w["x%d.n.w" % i], w["x%d.n.b" % i],

@@ -73,6 +73,41 @@ class PhiModel:
             f = F.linear(f, w["%d.fc2.w" % i], w["%d.fc2.b" % i])
         return kernels.add_layer_norm(h, w["fln.w"], w["fln.b"], cfg.eps, r1=a, r2=f)
 
+    def forward_suffix(self, inputs_embeds, prefix_cache, key_valid=None):
+        """Prefill of B prompt suffixes behind one shared prefix whose K / V rows of every layer are in `prefix_cache` (a
+        generate.PagedKVCache of one sequence and one page, filled by `forward(..., cache=...)` and advanced by its length
+        P).  inputs_embeds [B,Ts,C] are positions P..P+Ts-1; key_valid [B,Ts] (True/1 = real token) or None ->
+        last_hidden_state [B,Ts,C], the rows the unsplit prompts would give at those positions."""
+        cfg, w = self.cfg, self.w
+        B, T, C = inputs_embeds.shape
+        nh, hd = cfg.heads, cfg.head_dim
+        rd = int(hd * cfg.rotary_frac)
+        P = prefix_cache.length
+        key = ("suffix", P, T)
+        if key not in self._rope:    # rotary tables of positions P..P+Ts-1 (the kernel takes tables of any length)
+            cos, sin = self.rope_tables(P + T)
+            self._rope[key] = (cos[P:].contiguous(), sin[P:].contiguous())
+        cos, sin = self._rope[key]
+        kv = None
+        if key_valid is not None:
+            kv = key_valid.to(device=self.device, dtype=torch.uint8).contiguous()
+        h = inputs_embeds.contiguous()
+        a = f = None
+        for i in range(cfg.layers):
+            if a is None:
+                x = kernels.add_layer_norm(h, w["%d.ln.w" % i], w["%d.ln.b" % i], cfg.eps)
+            else:
+                h, x = kernels.add_layer_norm(h, w["%d.ln.w" % i], w["%d.ln.b" % i], cfg.eps, r1=a, r2=f, return_sum=True)
+            qkv = F.linear(x, w["%d.qkv.w" % i], w["%d.qkv.b" % i]).view(B, T, 3, nh, hd)
+            kernels.rotary_inplace(qkv, cos, sin, B, T, nh, hd, rd)
+            # prefix pages: [1 page, nh, page_size, hd] -> head-major [nh, page_size, hd]
+            a = kernels.timed("prefix_causal_attention", kernels.prefix_causal_attention, qkv, prefix_cache.k[i][0],
+                              prefix_cache.v[i][0], P, kv, B, T, nh, hd)
+            a = F.linear(a, w["%d.dense.w" % i], w["%d.dense.b" % i])
+            f = self._fc1_gelu(x, i)
+            f = F.linear(f, w["%d.fc2.w" % i], w["%d.fc2.b" % i])
+        return kernels.add_layer_norm(h, w["fln.w"], w["fln.b"], cfg.eps, r1=a, r2=f)
+
     def decode_step(self, x, cache):
         """One autoregressive step: x [B,1,C] = embedding of the newest token of every sequence, position cache.length
         (all sequences have the same length).  Appends its K / V to the cache and returns the final hidden state [B,1,C].

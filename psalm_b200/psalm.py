@@ -75,7 +75,95 @@ class PendingSeg:
         return results
 
 
+class PendingPrompts(PendingSeg):
+    """Handle of a submitted `ImageSession.eval_seg_async` call: `result()` post-processes every prompt's masks (one
+    image, K prompts) and returns what `ImageSession.eval_seg` returns."""
+
+    def __init__(self, model, outs, image_hw, seg_info, boxes, done, thing_lists, thresholds, mask_format):
+        super().__init__(model, None, image_hw, seg_info, boxes, done, None, None, thresholds, mask_format)
+        self.outs, self.thing_lists = outs, thing_lists
+
+    def result(self):
+        m = self.model
+        torch.cuda.current_stream(m.device).wait_event(self.done)
+        keep = (getattr(m, "is_thing_list", None), m.object_mask_threshold, m.overlap_threshold)
+        results = []
+        try:
+            m.object_mask_threshold, m.overlap_threshold = self.thresholds
+            for out, things in zip(self.outs, self.thing_lists):
+                m.is_thing_list = things
+                results += m.post_process(out, self.image_hw, self.seg_info, self.boxes)
+        finally:
+            m.is_thing_list, m.object_mask_threshold, m.overlap_threshold = keep
+        if self.mask_format == "rle":
+            attach_rle(results)
+        return results
+
+
+class ImageSession:
+    """One image opened by `PSALM.open_image`: its Swin maps, projector tokens, pixel-decoder outputs and decoder K / V
+    projections are computed once, and the prompt-independent prefix of every prompt set is prefilled once (its K / V
+    of all layers kept for the two most recent prefixes).  `eval_seg(prompts)` then runs only the prompt suffixes.
+    Valid until the next `open_image` on the same lane (a stale session raises RuntimeError)."""
+
+    MAX_PREFIXES = 2
+
+    def __init__(self, model, lane, gen, state, image_hw, seg_info, boxes):
+        self.model, self.lane, self.gen, self.state = model, lane, gen, state
+        self.image_hw, self.seg_info, self.boxes = image_hw, seg_info, boxes
+        self.prefixes = OrderedDict()     # prefix input ids (bytes) -> PagedKVCache of its K / V
+
+    def _check(self):
+        if self.model._lane_gen.get(self.lane) != self.gen:
+            raise RuntimeError("stale ImageSession: open_image was called again on lane %d" % self.lane)
+
+    def prefix_cache(self, split):
+        """K / V of the shared prefix `split` (prefilled on first use, two most recent prefixes kept)."""
+        key = split.prefix_ids.tobytes()
+        cache = self.prefixes.get(key)
+        if cache is None:
+            cache = self.model._prefix_for(self, split)
+            while len(self.prefixes) >= self.MAX_PREFIXES:
+                self.prefixes.popitem(last=False)
+            self.prefixes[key] = cache
+        self.prefixes.move_to_end(key)
+        return cache
+
+    @torch.no_grad()
+    def eval_seg(self, prompts, is_thing_list=None, mask_format="dense"):
+        """results[k] == model.eval_seg(images, seg_info, **prompts[k])[0] (same structure; values within the tolerances
+        of a split prefill).  A prompt dict may carry its own `is_thing_list` (panoptic prompts with different class
+        lists); it overrides the call-level one."""
+        return self.eval_seg_async(prompts, is_thing_list, mask_format).result()
+
+    @torch.no_grad()
+    def eval_seg_async(self, prompts, is_thing_list=None, mask_format="dense"):
+        if mask_format not in MASK_FORMATS:
+            raise ValueError("mask_format must be one of %s, got %r" % (MASK_FORMATS, mask_format))
+        self._check()
+        m = self.model
+        things = [p.get("is_thing_list", is_thing_list) for p in prompts]
+        if m.panoptic_on and any(t is None for t in things):
+            raise ValueError("is_thing_list need to be given")   # llava_phi.py:1337-1339
+        split, plan = m._cached_split(prompts, self.image_hw)
+        outs = m._prompts_forward(self, split, plan)
+        done = torch.cuda.Event()
+        done.record(torch.cuda.current_stream(m.device))
+        return PendingPrompts(m, outs, self.image_hw, self.seg_info[:1], self.boxes[:1], done, things,
+                              (m.object_mask_threshold, m.overlap_threshold), mask_format)
+
+
 MASK_FORMATS = ("dense", "rle")
+
+
+def _content_key(t):
+    """Hashable key of a prompt tensor (or a list of them) by content: the plan caches are keyed by what the prompt says."""
+    if t is None:
+        return None
+    if isinstance(t, (list, tuple)):
+        return tuple(_content_key(x) for x in t)
+    t = torch.as_tensor(t).detach().cpu().contiguous()
+    return (tuple(t.shape), str(t.dtype), t.numpy().tobytes())
 
 
 def attach_rle(results):
@@ -428,6 +516,211 @@ class PSALM:
         g.replay()
         return static_out
 
+    # ---- several prompts against one image ------------------------------------------------------------------------
+    @torch.no_grad()
+    def open_image(self, images, seg_info, lane=0):
+        """Encode ONE image (images [1,3,H,W]: float, uint8 or StagedImages, as eval_seg) for several prompts: Swin, the
+        projector, the pixel decoder and the decoder's K / V projections run once; returns an `ImageSession` whose
+        `eval_seg(prompts)` runs only what depends on the prompts.  Opening an image ends the previous session of `lane`."""
+        if images.shape[0] != 1 or len(seg_info) != 1:
+            raise ValueError("open_image takes one image (got %d)" % images.shape[0])
+        staged = images if isinstance(images, StagedImages) else None
+        if staged is not None:
+            torch.cuda.current_stream(self.device).wait_event(staged.ready)
+            images_d = staged.tensor
+        else:
+            images_d = images.to(self.device, non_blocking=True)
+        if not hasattr(self, "_lane_gen"):
+            self._lane_gen = {}
+        gen = self._lane_gen[lane] = self._lane_gen.get(lane, 0) + 1
+        if self.use_cuda_graph:
+            state = self._image_graphed(images_d, lane)
+        else:
+            with self._precision_scope():
+                state = self._image_core(images_d)
+        if staged is not None:
+            staged.slot[1] = torch.cuda.Event()
+            staged.slot[1].record(torch.cuda.current_stream(self.device))
+        _, boxes = self._fused_applies(images.shape[-2:], seg_info)
+        return ImageSession(self, lane, gen, state, tuple(images.shape[-2:]), list(seg_info), boxes)
+
+    def _image_core(self, images):
+        """Prompt-independent device work of one image (capturable)."""
+        toks, sizes = self.model.vision_tower.forward_tokens(images)
+        h5, w5 = sizes[3]
+        img_tok = self.model.mm_projector(toks[3].view(toks[3].shape[0], h5, w5, -1).permute(0, 3, 1, 2))
+        mask_features, ms, ms_sizes = self.pixel_decoder.forward_tokens(toks, sizes)
+        mem = self.predictor.memory(ms, ms_sizes, mask_features, sizes[0], self.num_queries)
+        return dict(swin=toks, swin_sizes=sizes, img_tok=img_tok, mask_features=mask_features, ms=ms, ms_sizes=ms_sizes,
+                    mem=mem, mask_size=sizes[0])
+
+    def _prefix_core(self, state, split, cache=None):
+        """Prefill of the shared prefix (split.tok_ids / img_pos on the device): its K / V of every layer in a one-page
+        PagedKVCache whose page holds the P rows rounded up to 64 (head-major [nh, P_pad, hd] per layer, the layout
+        psalm_prefix_causal_attention reads).  Capturable when `cache` is given (allocated and advanced by the caller)."""
+        from .generate import PagedKVCache
+        fresh = cache is None
+        if fresh:
+            page = -(-split.P // 64) * 64
+            cache = PagedKVCache(self.cfg.phi, 1, page, self.dtype, self.device, page_size=page)
+        with self._precision_scope():
+            self.model.phi.forward(SEQ.prefix_embeds(split, self.model.embed_tokens, state["img_tok"]), None, cache=cache)
+        if fresh:
+            cache.advance(split.P)
+        return cache
+
+    def _prompts_core(self, state, cache, plan):
+        """Device work of K prompt suffixes (plan on device) against an opened image and its prefix cache (capturable).
+        Returns forward_core's dict for the K prompts (pred_masks [K,Q,H4*W4], ...) and the suffix hidden states."""
+        with self._precision_scope():
+            img_tok = state["img_tok"]
+            embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok[:, :0], self.seg_query)
+            hidden = self.model.phi.forward_suffix(embeds, cache, plan.attention_mask if plan.any_padding else None)
+            seg_q = F.linear(SEQ.gather_seg_query(plan, hidden), *self.proj["seg_query_projector"])
+            SEG_emb = cls_emb = None
+            if plan.refer_pool is not None:
+                SEG_emb = F.linear(SEQ.pool(plan.refer_pool, hidden), *self.proj["SEG_token_projector"])
+            if plan.cls_pool is not None:
+                cls_emb = F.linear(SEQ.pool(plan.cls_pool, hidden), *self.proj["class_name_projector"])
+            out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
+                                                memory=state["mem"])
+            out["mask_size"] = state["mask_size"]
+            out["hidden"], out["seg_query"] = hidden, seg_q
+            return out
+
+    def _cached_split(self, prompts, image_hw):
+        """(host PromptSplit, device suffix plan) of a prompt set, cached by content like `_cached_plan`."""
+        key = (tuple(image_hw),) + tuple(tuple(_content_key(p.get(n)) for n in SEQ.PROMPT_KEYS) for p in prompts)
+        if not hasattr(self, "_splits"):
+            self._splits = OrderedDict()
+        ent = self._splits.get(key)
+        if ent is None:
+            import dataclasses
+            split = SEQ.split_prompts(prompts, self.make_plan_n_img(image_hw), self.num_queries)
+            plan = split.suffix.to(self.device)
+            split = dataclasses.replace(split, tok_ids=split.tok_ids.to(self.device), img_pos=split.img_pos.to(self.device),
+                                        suffix=None)
+            ent = (split, plan)
+            while len(self._splits) >= 16:
+                self._splits.popitem(last=False)
+            self._splits[key] = ent
+        self._splits.move_to_end(key)
+        return ent
+
+    def make_plan_n_img(self, image_hw):
+        """Projector tokens of an image of size image_hw (the <image> expansion of make_plan)."""
+        H, W = image_hw
+        ps = self.cfg.swin.patch
+        h, w = -(-H // ps), -(-W // ps)
+        for _ in range(len(self.cfg.swin.depths) - 1):
+            h, w = (h + 1) // 2, (w + 1) // 2
+        return ((h - 1) // 2 + 1) * ((w - 1) // 2 + 1)   # conv3x3 stride 2 pad 1 of the projector
+
+    # CUDA graphs of the session phases: the image (per lane, image shape and dtype), the prefix prefill (per lane, image
+    # key and prefix content) and the prompt pass (per lane, prefix, K, suffix length and plan structure, task heads).
+    # Later phases read the static buffers of the earlier ones of the same lane, so a session is valid until the next
+    # open_image on its lane.  Bounded LRUs like MAX_GRAPHS.
+    MAX_SESSION_GRAPHS = 8
+
+    def _capture(self, fn):
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(side), self._precision_scope():
+            for _ in range(2):
+                fn()
+        torch.cuda.current_stream(self.device).wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        g = torch.cuda.CUDAGraph()
+        with self._precision_scope(), torch.cuda.graph(g):
+            out = fn()
+        return g, out
+
+    def _session_graph(self, table, key, make):
+        graphs = self.__dict__.setdefault(table, OrderedDict())
+        ent = graphs.get(key)
+        if ent is None:
+            ent = make()
+            while len(graphs) >= self.MAX_SESSION_GRAPHS:
+                graphs.popitem(last=False)
+            graphs[key] = ent
+        graphs.move_to_end(key)
+        return ent
+
+    def _image_graphed(self, images, lane):
+        key = (lane, tuple(images.shape), str(images.dtype))
+
+        def make():
+            static_img = images.clone()
+            g, state = self._capture(lambda: self._image_core(static_img))
+            return g, static_img, state
+        g, static_img, state = self._session_graph("_image_graphs", key, make)
+        static_img.copy_(images, non_blocking=True)
+        g.replay()
+        return state
+
+    def _prefix_for(self, sess, split):
+        if not self.use_cuda_graph:
+            return self._prefix_core(sess.state, split)
+        # keyed by the image graph's state object: a re-captured image graph has new buffers; entries keep what they read
+        key = (sess.lane, id(sess.state), split.prefix_ids.tobytes())
+
+        def make():
+            import dataclasses
+            from .generate import PagedKVCache
+            page = -(-split.P // 64) * 64
+            cache = PagedKVCache(self.cfg.phi, 1, page, self.dtype, self.device, page_size=page)
+            # the graph reads its own copies of the prefix rows' token ids and image rows (the split that brought them
+            # lives in a bounded cache and may be freed); they are refreshed before every replay
+            static = dataclasses.replace(split, tok_ids=split.tok_ids.clone(), img_pos=split.img_pos.clone())
+            g, _ = self._capture(lambda: self._prefix_core(sess.state, static, cache))
+            # the replayed writes start at seq_lens (0): only the host-side length moves (forward_suffix reads it)
+            cache.length = split.P
+            return g, cache, sess.state, static
+        g, cache, _, static = self._session_graph("_prefix_graphs", key, make)
+        static.tok_ids.copy_(split.tok_ids, non_blocking=True)
+        static.img_pos.copy_(split.img_pos, non_blocking=True)
+        g.replay()
+        return cache
+
+    _PLAN_TENSORS = ("tok_ids", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool")
+
+    def _prompts_graphed(self, sess, cache, split, plan):
+        key = (sess.lane, id(sess.state), id(cache), plan.B, plan.T, plan.any_padding,
+               None if plan.cls_pool is None else tuple(plan.cls_pool.shape), plan.refer_pool is not None,
+               None if plan.pad_pos is None else int(plan.pad_pos.numel()), self.seg_task)
+
+        def make():
+            import copy
+            static_plan = copy.copy(plan)
+            for n in self._PLAN_TENSORS:
+                t = getattr(plan, n)
+                setattr(static_plan, n, None if t is None else t.clone())
+            g, out = self._capture(lambda: self._prompts_core(sess.state, cache, static_plan))
+            return g, static_plan, out, (sess.state, cache)
+        g, static_plan, out, _ = self._session_graph("_prompt_graphs", key, make)
+        for n in self._PLAN_TENSORS:
+            t = getattr(plan, n)
+            if t is not None:
+                getattr(static_plan, n).copy_(t, non_blocking=True)
+        g.replay()
+        return out
+
+    def _prompts_forward(self, sess, split, plan):
+        """Run the prompt pass of a session and cut its output into one forward_core-style dict per prompt."""
+        cache = sess.prefix_cache(split)
+        if self.use_cuda_graph:
+            out = self._prompts_graphed(sess, cache, split, plan)
+        else:
+            out = self._prompts_core(sess.state, cache, plan)
+        outs = []
+        for k, ncls in enumerate(split.n_classes):
+            cls = out["pred_class_name_logits"]
+            seg = out["pred_SEG_logits"]
+            outs.append(dict(pred_masks=out["pred_masks"][k:k + 1], mask_size=out["mask_size"],
+                             pred_class_name_logits=None if cls is None else cls[k:k + 1, :, :ncls].contiguous(),
+                             pred_SEG_logits=None if seg is None else seg[k:k + 1]))
+        return outs
+
     # ---- input staging: overlap the upload of batch k+1 with the compute of batch k ----------------------
     def stage_images(self, images_host):
         """Enqueue the host->device copy of a (pinned) image batch on a dedicated copy stream and return a
@@ -452,27 +745,14 @@ class PSALM:
 
     def make_plan(self, input_ids, attention_mask, image_hw, class_name_ids=None, cls_indices=None,
                   class_name_embedding_indices=None, token_refer_id=None, refer_embedding_indices=None):
-        H, W = image_hw
-        ps = self.cfg.swin.patch
-        h, w = -(-H // ps), -(-W // ps)
-        for _ in range(len(self.cfg.swin.depths) - 1):
-            h, w = (h + 1) // 2, (w + 1) // 2
-        n_img = ((h - 1) // 2 + 1) * ((w - 1) // 2 + 1)   # conv3x3 stride 2 pad 1 of the projector
-        return SEQ.build_plan(input_ids, attention_mask, n_img, self.num_queries, class_name_ids, cls_indices,
+        return SEQ.build_plan(input_ids, attention_mask, self.make_plan_n_img(image_hw), self.num_queries, class_name_ids, cls_indices,
                               class_name_embedding_indices, token_refer_id, refer_embedding_indices)
 
     def _cached_plan(self, input_ids, attention_mask, image_hw, class_name_ids, cls_indices,
                      class_name_embedding_indices, token_refer_id, refer_embedding_indices):
         """The sequence plan depends only on the prompt (ids / masks / class-name tables) and the image size;
         evaluation loops reuse one prompt for every image, so the device-resident plan is cached by content."""
-        def key_of(t):
-            if t is None:
-                return None
-            if isinstance(t, (list, tuple)):
-                return tuple(key_of(x) for x in t)
-            t = t.detach().cpu().contiguous()
-            return (tuple(t.shape), str(t.dtype), t.numpy().tobytes())
-        key = (tuple(image_hw),) + tuple(key_of(t) for t in (input_ids, attention_mask, class_name_ids, cls_indices,
+        key = (tuple(image_hw),) + tuple(_content_key(t) for t in (input_ids, attention_mask, class_name_ids, cls_indices,
                                                               class_name_embedding_indices, token_refer_id,
                                                               refer_embedding_indices))
         if not hasattr(self, "_plans"):

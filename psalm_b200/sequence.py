@@ -52,8 +52,10 @@ class SequencePlan:
 
 
 def build_plan(input_ids, attention_mask, n_img, n_q, class_name_ids=None, cls_indices=None,
-               class_name_embedding_indices=None, token_refer_id=None, refer_embedding_indices=None):
-    """All arguments are HOST tensors in the reference's input contract (train_datasets.py:186-234)."""
+               class_name_embedding_indices=None, token_refer_id=None, refer_embedding_indices=None, suffix=False):
+    """All arguments are HOST tensors in the reference's input contract (train_datasets.py:186-234).
+    suffix=True: the rows are prompt suffixes behind a shared prefix that holds the <image> (split_prompts); they carry
+    no <image> sentinel, and a class list may be shorter than the longest of the batch (its extra pooling rows are 0)."""
     ids_all = input_ids.cpu().numpy()
     B, T0 = ids_all.shape
     am_all = np.ones((B, T0), bool) if attention_mask is None else attention_mask.cpu().numpy().astype(bool)
@@ -61,7 +63,7 @@ def build_plan(input_ids, attention_mask, n_img, n_q, class_name_ids=None, cls_i
     rows = []
     for b in range(B):
         ids = ids_all[b]
-        assert (ids == IMAGE_TOKEN_INDEX).sum() == 1, "not supporting multi image index"   # llava_phi.py:588
+        assert (ids == IMAGE_TOKEN_INDEX).sum() == (0 if suffix else 1), "not supporting multi image index"   # llava_phi.py:588
         assert (ids == SEG_TOKEN_INDEX).sum() == 1, "not supporting multi seg index"       # llava_phi.py:589
         names = None
         if class_name_ids is not None:  # embed_class_ids, llava_phi.py:566-575
@@ -140,6 +142,8 @@ def build_plan(input_ids, attention_mask, n_img, n_q, class_name_ids=None, cls_i
         for b in range(B):
             for c in range(1, ncls + 1):
                 m = cls_idx[b] == c
+                if suffix and not m.any():   # a shorter class list than the batch's longest
+                    continue
                 assert m.any(), "class %d has no tokens in sample %d" % (c, b)
                 cls_pool[b, c - 1, m] = 1.0 / m.sum()   # AdaptiveAvgPool1d(1), llava_phi.py:561-563
     if refer_embedding_indices is not None:
@@ -185,3 +189,118 @@ def pool(pool_matrix, hidden):
 def gather_region_rows(plan, hidden):
     """hidden [B,T,C] -> [R,C] hidden states at the <region> positions (get_region_embedding, llava_phi.py:302-307)."""
     return hidden.reshape(plan.B * plan.T, -1).index_select(0, plan.region_pos)
+
+
+# ---- several prompts against one image: shared prefix + per-prompt suffixes ---------------------------------------
+OUTPUT_SENTINELS = (SEG_TOKEN_INDEX, CLS_TOKEN_INDEX, REFER_TOKEN_INDEX, REGION_TOKEN_INDEX)
+PROMPT_KEYS = ("input_ids", "attention_mask", "token_refer_id", "refer_embedding_indices", "class_name_ids", "cls_indices",
+               "class_name_embedding_indices")
+
+
+@dataclass
+class PromptSplit:
+    prefix_ids: np.ndarray      # [L] int64 input ids of the shared prefix (holds the <image> sentinel)
+    P: int                      # rows of the prefix after the <image> expansion
+    tok_ids: torch.Tensor       # [1,P] int64 token id of every prefix row (0 on image rows)
+    img_pos: torch.Tensor       # [n_img] int64 prefix rows of the image tokens
+    suffix: SequencePlan        # [K, Ts] plan of the remaining tokens of every prompt (right padded)
+    n_classes: tuple            # classes of every prompt (0 without a class list)
+
+
+def _row(t, name):
+    """One prompt's tensor: [T] or [1, T] (a list / tuple of one tensor for token_refer_id) -> host 1-D tensor."""
+    if t is None:
+        return None
+    if isinstance(t, (list, tuple)):
+        if len(t) != 1:
+            raise ValueError("%s: one prompt per dict (got %d rows)" % (name, len(t)))
+        t = t[0]
+    t = torch.as_tensor(t).cpu()
+    if t.dim() == 2:
+        if t.shape[0] != 1:
+            raise ValueError("%s: one prompt per dict (got %d rows)" % (name, t.shape[0]))
+        t = t[0]
+    return t
+
+
+def split_prompts(prompts, n_img, n_q):
+    """Cut K prompts of one image into the shared prefix and K suffixes (input_ids space).  The prefix is the longest
+    common token prefix of the prompts, truncated at the first position that feeds an output (a <seg>, <cls>, <refer> or
+    <region> sentinel, or a non-zero class-name / refer embedding index).  It must hold the <image> sentinel and no masked
+    position.  Raises ValueError (or NotImplementedError for <region> prompts) instead of falling back."""
+    if not prompts:
+        raise ValueError("no prompts")
+    rows = []
+    for k, p in enumerate(prompts):
+        unknown = set(p) - set(PROMPT_KEYS) - {"is_thing_list"}
+        if unknown:
+            raise ValueError("prompt %d: unknown keys %s" % (k, sorted(unknown)))
+        r = {n: _row(p.get(n), n) for n in PROMPT_KEYS if n not in ("class_name_ids", "cls_indices", "token_refer_id")}
+        r["ids"] = r.pop("input_ids").numpy().astype(np.int64)
+        if (r["ids"] == REGION_TOKEN_INDEX).any():
+            raise NotImplementedError("<region> prompts pool their features per prompt from sampled points; they are not "
+                                      "supported by multi-prompt sessions")
+        T0 = len(r["ids"])
+        r["am"] = np.ones(T0, bool) if r["attention_mask"] is None else r["attention_mask"].numpy().astype(bool)
+        r["cei"] = None if r["class_name_embedding_indices"] is None else r["class_name_embedding_indices"].numpy()
+        r["rei"] = None if r["refer_embedding_indices"] is None else r["refer_embedding_indices"].numpy()
+        for n in ("class_name_ids", "cls_indices", "token_refer_id"):
+            r[n] = _row(p.get(n), n)
+        rows.append(r)
+    for n in ("class_name_ids", "token_refer_id", "cei", "rei"):
+        if len({rows[k][n] is None for k in range(len(rows))}) > 1:
+            raise ValueError("prompts of one call must all have or all lack %s" % n)
+    ids0 = rows[0]["ids"]
+    L = min(len(r["ids"]) for r in rows)
+    for r in rows[1:]:
+        neq = np.nonzero(r["ids"][:L] != ids0[:L])[0]
+        if len(neq):
+            L = int(neq[0])
+    feeds = np.isin(ids0[:L], OUTPUT_SENTINELS)
+    for r in rows:
+        for n in ("cei", "rei"):
+            if r[n] is not None:
+                feeds |= r[n][:L] != 0
+    if feeds.any():
+        L = int(np.nonzero(feeds)[0][0])
+    img = np.nonzero(ids0[:L] == IMAGE_TOKEN_INDEX)[0]
+    if len(img) != 1:
+        raise ValueError("the shared prefix of the prompts (%d tokens) does not contain the <image> sentinel: the prompts "
+                         "differ, or feed an output, before <image>" % L)
+    for k, r in enumerate(rows):
+        if not r["am"][:L].all():
+            raise ValueError("prompt %d has a masked position inside the shared prefix (first %d tokens)" % (k, L))
+    i0 = int(img[0])
+    P = L - 1 + n_img
+    tok = np.concatenate([ids0[:i0], np.zeros(n_img, np.int64), ids0[i0 + 1:L]])
+    Ts0 = max(len(r["ids"]) - L for r in rows)
+    K = len(rows)
+    ids = np.zeros((K, Ts0), np.int64)
+    am = np.zeros((K, Ts0), bool)
+    cei = np.zeros((K, Ts0), np.int64) if rows[0]["cei"] is not None else None
+    rei = np.zeros((K, Ts0), np.int64) if rows[0]["rei"] is not None else None
+    for k, r in enumerate(rows):
+        n = len(r["ids"]) - L
+        ids[k, :n], am[k, :n] = r["ids"][L:], r["am"][L:]
+        if cei is not None:
+            cei[k, :n] = r["cei"][L:]
+        if rei is not None:
+            rei[k, :n] = r["rei"][L:]
+    ft = torch.from_numpy
+    has_cls = rows[0]["class_name_ids"] is not None
+    plan = build_plan(ft(ids), ft(am), n_img, n_q,
+                      [r["class_name_ids"] for r in rows] if has_cls else None,
+                      [r["cls_indices"] for r in rows] if has_cls else None,
+                      ft(cei) if cei is not None else None,
+                      [r["token_refer_id"] for r in rows] if rows[0]["token_refer_id"] is not None else None,
+                      ft(rei) if rei is not None else None, suffix=True)
+    n_classes = tuple(int((ids[k] == CLS_TOKEN_INDEX).sum()) for k in range(K))
+    return PromptSplit(ids0[:L].copy(), P, ft(tok).view(1, P), ft(i0 + np.arange(n_img, dtype=np.int64)), plan, n_classes)
+
+
+def prefix_embeds(split, embed_tokens, image_tokens):
+    """Shared prefix rows [1,P,C]: token embeddings with the projector tokens image_tokens [1,n_img,C] at the image rows."""
+    C = embed_tokens.shape[1]
+    flat = embed_tokens.index_select(0, split.tok_ids.view(-1))
+    flat.index_copy_(0, split.img_pos, image_tokens.reshape(-1, C).to(flat.dtype))
+    return flat.view(1, split.P, C)
