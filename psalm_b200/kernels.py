@@ -396,13 +396,12 @@ def region_pool(tokens, points, region_image, h, w):
     return out
 
 
-LINEAR_FUSED = True   # False: library GEMM + separate elementwise pass (A/B runs)
 _EPILOGUES = {"bias": 0, "gelu_erf": 1, "head_major": 2}
 
 
 def linear_fused_supported(x, weight, epilogue, rows_per_image=0):
     """True when `linear_fused` applies: 16-bit CUDA tensors, N % 256 == 0, K % 64 == 0."""
-    if not (LINEAR_FUSED and x.is_cuda and x.dtype in (torch.bfloat16, torch.float16)):
+    if not (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16)):
         return False
     M = x.numel() // x.shape[-1]
     return bool(_lib.lib().psalm_linear_fused_supported(M, weight.shape[0], weight.shape[1], _EPILOGUES[epilogue],

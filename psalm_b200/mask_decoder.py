@@ -14,8 +14,6 @@ Mirrors `MultiScaleMaskedTransformerDecoderForOPTPreTrain.forward_woconcat`
     nine are thresholded and thrown away (236 MB of logits per image in the reference);
   * `(sigmoid(x) < 0.5)` is `x < 0`; fully blocked rows are opened by a per-row flag (:647).
 """
-import os
-
 import torch
 import torch.nn.functional as F
 
@@ -183,8 +181,7 @@ class MultiScaleMaskedTransformerDecoderForOPTPreTrain:
             return kernels.mask_bits(me.contiguous(), pooled[level])
 
         qc = None
-        fold_q = fused_kv and not os.environ.get("PSALM_NO_QCONST")
-        if fold_q:
+        if fused_kv:
             # (output + query_pos) W^T + b = output W^T + (query_pos W^T + b): the position terms of the cross-attention
             # query and of the self-attention query / key do not depend on the input; they enter the GEMMs as the additive
             # C matrix (no `output + query_pos` passes), and the self-attention K and V projections share one GEMM whose
@@ -209,7 +206,7 @@ class MultiScaleMaskedTransformerDecoderForOPTPreTrain:
             if hooks is not None:
                 output, bits, row_open = hooks.before_layer(i, output, bits, row_open, lambda o_, lv=li: mask_for(lv, o_))
             # masked cross-attention (:93-105): q = tgt + query_pos, k = memory + pos, v = memory
-            if fold_q:
+            if fused_kv:
                 q = torch.addmm(qc[i][0], output.reshape(-1, Hd), w["x%d.q.w" % i].t()).view(B, Q, Hd)
             else:
                 q = F.linear(output + qpos, w["x%d.q.w" % i], w["x%d.q.b" % i])
@@ -226,7 +223,7 @@ class MultiScaleMaskedTransformerDecoderForOPTPreTrain:
             output = kernels.add_layer_norm(output, w["x%d.n.w" % i], w["x%d.n.b" % i],
                                             r1=F.linear(a, w["x%d.o.w" % i], w["x%d.o.b" % i]))
             # query self-attention (:35-45): q = k = tgt + query_pos, v = tgt
-            if fold_q:
+            if fused_kv:
                 o2 = output.reshape(-1, Hd)
                 q = torch.addmm(qc[i][1], o2, w["s%d.q.w" % i].t()).view(B, Q, Hd)
                 kv = torch.addmm(qc[i][2], o2, qc[i][3].t()).view(B, Q, 2 * Hd)

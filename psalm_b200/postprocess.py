@@ -119,10 +119,21 @@ def panoptic_inference(cls, mask_pred, is_thing_list, obj_thr=0.8, ovl_thr=0.8, 
     inter = torch.bincount(ids, weights=in_mask.float(), minlength=Q).long()
     orig = (mask_pred >= 0).flatten(1).sum(1)
     host = torch.stack([keep.long(), labels.long(), area, orig, inter], 0).cpu().numpy()   # the one D2H copy
+    if host[0].sum() == 0:
+        return torch.zeros((H, W), dtype=torch.int32, device=cls.device), []
+    seg_of_query, info = panoptic_merge(host, is_thing_list, ovl_thr)
+    lut = torch.from_numpy(seg_of_query).to(cls.device)
+    pan = torch.where(in_mask, lut[ids], torch.zeros((), dtype=torch.int32, device=cls.device))
+    return pan.view(H, W).to(torch.int32), info
+
+
+def panoptic_merge(host, is_thing_list, ovl_thr):
+    """The reference's sequential merge rule (llava_phi.py:355-384) on the per-query integers host [5, Q] (rows: keep,
+    class, area, original area, intersection): stuff classes share one segment id, a query whose visible area is below
+    `ovl_thr` of its own mask is dropped.  Returns (seg_of_query int32 [Q], 0 = no segment; segments_info)."""
+    Q = host.shape[1]
     seg_of_query = np.zeros(Q, np.int32)
     info, stuff, cur = [], {}, 0
-    if host[0].sum() == 0:
-        return torch.zeros((H, W), dtype=torch.int32, device=cls.device), info
     for q in range(Q):
         if not host[0, q]:
             continue
@@ -139,9 +150,7 @@ def panoptic_inference(cls, mask_pred, is_thing_list, obj_thr=0.8, ovl_thr=0.8, 
             cur += 1
             seg_of_query[q] = cur
             info.append(dict(id=cur, isthing=isthing, category_id=pc))
-    lut = torch.from_numpy(seg_of_query).to(cls.device)
-    pan = torch.where(in_mask, lut[ids], torch.zeros((), dtype=torch.int32, device=cls.device))
-    return pan.view(H, W).to(torch.int32), info
+    return seg_of_query, info
 
 
 _THING_CACHE = {}
@@ -155,63 +164,19 @@ def thing_tensor(is_thing_list, device):
     return _THING_CACHE[key]
 
 
-def fused_device(kernels, logits, H, W, cls=None, SEG_cls=None, thing=None, semantic_on=False, instance_on=False,
-                 panoptic_on=False, referring_on=False, topk=100, obj_thr=0.8, crop=None):
-    """Device part of the fused task heads (no host synchronisation, CUDA-graph capturable): small
-    [Q, n_cls] tensor algebra in torch + ONE fused kernel (csrc/postproc.cu) on the LOW-RESOLUTION mask
-    logits [Q,H4,W4].  Returns device tensors plus `hostvec`, the one vector the host part needs."""
-    Q = logits.shape[0]
-    dev = logits.device
-    probsT = wq = negq = slots = None
-    ncls = 0
-    d = dict(Q=Q, H=H, W=W)
-    if cls is not None:
-        probs_full = F.softmax(cls.float(), dim=-1)
-        probs = probs_full[:, :-1]
-        ncls = probs.shape[1]
-    if semantic_on:
-        probsT = torch.zeros((144, 112), dtype=torch.float16, device=dev)
-        probsT[:ncls, :Q] = probs.t().to(torch.float16)
-    if panoptic_on:
-        scores, labels = probs_full.max(-1)
-        keep = labels.ne(ncls) & (scores > obj_thr)
-        wq = torch.where(keep, scores, torch.zeros_like(scores)).contiguous()
-        negq = (keep.float() - 1.0).contiguous()
-    s = lab = qi = keep_i = None
-    if instance_on:
-        s, idx = probs.flatten(0, 1).topk(topk, sorted=False)
-        lab, qi = idx % ncls, idx // ncls
-        if panoptic_on:
-            keep_i = thing[lab]
-            order = torch.sort((~keep_i).to(torch.uint8), stable=True).indices      # kept slots first
-            s, lab, qi, keep_i = s[order], lab[order], qi[order], keep_i[order]
-        else:
-            keep_i = torch.ones_like(qi, dtype=torch.bool)
-        slots = torch.where(keep_i, qi, torch.full_like(qi, -1)).to(torch.int32).contiguous()
-    elif referring_on:
-        s, qi = torch.sigmoid(SEG_cls.float()).flatten(0, 1).topk(topk, sorted=False)
-        keep_i = torch.ones_like(qi, dtype=torch.bool)
-        slots = qi.to(torch.int32).contiguous()
-    k = kernels.postproc_fused(logits.contiguous(), H, W, probsT, wq, negq, slots, ncls, crop=crop)
-    st = k["stats"]
-    d.update(sem_seg=k["sem_seg"], inst_masks=k["inst_masks"], ids=k["ids"], in_mask=k["in_mask"], lab=lab, qi=qi)
-    rows = []
-    if slots is not None:
-        rows.append(keep_i.sum().view(1).float())
-        d["inst_scores"] = s * (st[:, 1] / (st[:, 0] + 1e-6))[qi]               # class score x per-query mask score
-    if panoptic_on:
-        rows += [keep.float(), labels.float(), st[:, 3], st[:, 2], st[:, 4]]
-    d["hostvec"] = torch.cat(rows) if rows else None
-    d["has_inst"], d["has_pan"], d["has_sem"] = slots is not None, bool(panoptic_on), bool(semantic_on)
-    return d
+# Limits of the fused task-head kernel (csrc/postproc.cu): at most 104 queries and 144 classes; its class-probability
+# operand `probsT` is fp16 [144, 112], zero padded (queries padded to 112).
+FUSED_MAX_QUERIES, FUSED_MAX_CLASSES, FUSED_PADDED_QUERIES = 104, 144, 112
 
 
 def fused_device_batch(kernels, logits, sizes, cls=None, SEG_cls=None, thing=None, semantic_on=False, instance_on=False,
                        panoptic_on=False, referring_on=False, topk=100, obj_thr=0.8, crops=None):
-    """`fused_device` for a whole batch: the small [Q, n_cls] algebra (softmax, arg-max, top-k, stable partition of the
-    kept slots) runs ONCE on [B, ...] tensors instead of once per image (~25 tiny launches per image, among them a
-    57 us single-block top-k), then one fused kernel per image.  logits [B,Q,H4,W4]; sizes / crops: per image (H, W) and
-    None | (Hp, Wp, oh, ow).  Returns the list of per-image dicts `fused_host` consumes."""
+    """Device part of the fused task heads for a batch (no host synchronisation, CUDA-graph capturable): the small
+    [Q, n_cls] algebra (softmax, arg-max, top-k, stable partition of the kept slots) runs ONCE on [B, ...] tensors
+    instead of once per image (~25 tiny launches per image, among them a 57 us single-block top-k), then one fused kernel
+    (csrc/postproc.cu) per image on its LOW-RESOLUTION mask logits.  logits [B,Q,H4,W4]; sizes / crops: per image (H, W)
+    and None | (Hp, Wp, oh, ow).  Returns the list of per-image dicts `fused_host` consumes; each holds `hostvec`, the
+    one vector its host part needs."""
     B, Q = logits.shape[:2]
     dev = logits.device
     probsT = wq = negq = slots = None
@@ -221,7 +186,7 @@ def fused_device_batch(kernels, logits, sizes, cls=None, SEG_cls=None, thing=Non
         probs = probs_full[..., :-1]
         ncls = probs.shape[-1]
     if semantic_on:
-        probsT = torch.zeros((B, 144, 112), dtype=torch.float16, device=dev)
+        probsT = torch.zeros((B, FUSED_MAX_CLASSES, FUSED_PADDED_QUERIES), dtype=torch.float16, device=dev)
         probsT[:, :ncls, :Q] = probs.transpose(1, 2).to(torch.float16)
     if panoptic_on:
         scores, labels = probs_full.max(-1)
@@ -296,38 +261,11 @@ def fused_host(d, is_thing_list=None, ovl_thr=0.8, host=None):
     if d["has_pan"]:
         dev = d["ids"].device
         hk = host[pos:].reshape(5, Q)
-        seg_of_query = np.zeros(Q, np.int32)
-        info, stuff, cur = [], {}, 0
-        for q in range(Q):
-            if not hk[0, q]:
-                continue
-            pc, a, o, it = int(hk[1, q]), int(hk[2, q]), int(hk[3, q]), int(hk[4, q])
-            if a > 0 and o > 0 and it > 0:
-                if a / o < ovl_thr:
-                    continue
-                isthing = bool(is_thing_list[pc])
-                if not isthing:
-                    if pc in stuff:
-                        seg_of_query[q] = stuff[pc]
-                        continue
-                    stuff[pc] = cur + 1
-                cur += 1
-                seg_of_query[q] = cur
-                info.append(dict(id=cur, isthing=isthing, category_id=pc))
         if hk[0].sum() == 0:
-            pan = torch.zeros((H, W), dtype=torch.int32, device=dev)
+            pan, info = torch.zeros((H, W), dtype=torch.int32, device=dev), []
         else:
+            seg_of_query, info = panoptic_merge(hk, is_thing_list, ovl_thr)
             lut = torch.from_numpy(seg_of_query).to(dev)
             pan = torch.where(d["in_mask"].bool(), lut[d["ids"].long()], torch.zeros((), dtype=torch.int32, device=dev))
         r["panoptic_seg"] = (pan.to(torch.int32), info)
     return r
-
-
-def fused_postprocess(kernels, logits, H, W, cls=None, SEG_cls=None, is_thing_list=None, semantic_on=False,
-                      instance_on=False, panoptic_on=False, referring_on=False, topk=100, obj_thr=0.8, ovl_thr=0.8, crop=None):
-    """All task heads of one image from the LOW-RESOLUTION mask logits with one fused kernel — same results
-    as the step-by-step functions above applied to the up-sampled [Q,H,W] map, which is never materialised."""
-    thing = thing_tensor(is_thing_list, logits.device) if (panoptic_on and instance_on) else None
-    d = fused_device(kernels, logits, H, W, cls, SEG_cls, thing, semantic_on, instance_on, panoptic_on, referring_on,
-                     topk, obj_thr, crop=crop)
-    return fused_host(d, is_thing_list, ovl_thr)

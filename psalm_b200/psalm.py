@@ -20,9 +20,8 @@ How it differs from the reference on purpose (results are unchanged, see DESIGN.
   * no CPU / PyTorch fallback for the hot operators: a missing CUDA library raises.
 """
 import contextlib
+import copy
 from collections import OrderedDict
-
-import os
 
 import torch
 import torch.nn.functional as F
@@ -48,53 +47,29 @@ class StagedImages:
 
 
 class PendingSeg:
-    """Handle of a submitted `PSALM.eval_seg_async` call: the network + the device part of the task heads are queued
-    (one graph replay), the few integers the host merge needs are on their way to pinned memory.  `result()` finishes
-    the post-processing ON THE CALLER'S CURRENT STREAM (after making it wait for the pass), so a caller that wants the
-    host work of image batch k to overlap the device work of batch k+1 submits k+1 first and calls `result()` of k
-    under a side stream.  The tensors of the result live in the lane's static buffers: they stay valid until the next
-    submission on the same lane."""
+    """Handle of a submitted `PSALM.eval_seg_async` or `ImageSession.eval_seg_async` call: the device work is queued
+    (graph replays), and when the graph holds the device part of the task heads, the few integers the host merge needs
+    are on their way to pinned memory.  `result()` finishes the post-processing ON THE CALLER'S CURRENT STREAM (after
+    making it wait for the pass), so a caller that wants the host work of image batch k to overlap the device work of
+    batch k+1 submits k+1 first and calls `result()` of k under a side stream.  The tensors of the result live in the
+    lane's static buffers: they stay valid until the next submission on the same lane.
 
-    def __init__(self, model, out, image_hw, seg_info, boxes, done, hostvecs, thing_list, thresholds, mask_format="dense"):
-        self.model, self.out, self.image_hw, self.seg_info, self.boxes = model, out, image_hw, seg_info, boxes
-        self.done, self.hostvecs, self.thing_list, self.thresholds = done, hostvecs, thing_list, thresholds
-        self.mask_format = mask_format
+    `parts`: one (out, hostvecs, is_thing_list) per forward output (one for an image batch, one per prompt of a
+    session), post-processed with the `thresholds` (object mask, overlap) of the submission."""
 
-    def result(self):
-        m = self.model
-        torch.cuda.current_stream(m.device).wait_event(self.done)
-        self.done.synchronize()                              # pinned host vectors are complete
-        keep = (getattr(m, "is_thing_list", None), m.object_mask_threshold, m.overlap_threshold)
-        m.is_thing_list, (m.object_mask_threshold, m.overlap_threshold) = self.thing_list, self.thresholds
-        try:
-            results = m.post_process(self.out, self.image_hw, self.seg_info, self.boxes, hostvecs=self.hostvecs)
-        finally:
-            m.is_thing_list, m.object_mask_threshold, m.overlap_threshold = keep
-        if self.mask_format == "rle":
-            attach_rle(results)
-        return results
-
-
-class PendingPrompts(PendingSeg):
-    """Handle of a submitted `ImageSession.eval_seg_async` call: `result()` post-processes every prompt's masks (one
-    image, K prompts) and returns what `ImageSession.eval_seg` returns."""
-
-    def __init__(self, model, outs, image_hw, seg_info, boxes, done, thing_lists, thresholds, mask_format):
-        super().__init__(model, None, image_hw, seg_info, boxes, done, None, None, thresholds, mask_format)
-        self.outs, self.thing_lists = outs, thing_lists
+    def __init__(self, model, parts, image_hw, seg_info, boxes, done, thresholds, mask_format="dense"):
+        self.model, self.parts, self.image_hw, self.seg_info, self.boxes = model, parts, image_hw, seg_info, boxes
+        self.done, self.thresholds, self.mask_format = done, thresholds, mask_format
 
     def result(self):
         m = self.model
         torch.cuda.current_stream(m.device).wait_event(self.done)
-        keep = (getattr(m, "is_thing_list", None), m.object_mask_threshold, m.overlap_threshold)
-        results = []
-        try:
-            m.object_mask_threshold, m.overlap_threshold = self.thresholds
-            for out, things in zip(self.outs, self.thing_lists):
-                m.is_thing_list = things
-                results += m.post_process(out, self.image_hw, self.seg_info, self.boxes)
-        finally:
-            m.is_thing_list, m.object_mask_threshold, m.overlap_threshold = keep
+        if any(hostvecs is not None for _, hostvecs, _ in self.parts):
+            self.done.synchronize()                          # pinned host vectors are complete
+        results = None
+        for out, hostvecs, things in self.parts:
+            res = m.post_process(out, self.image_hw, self.seg_info, self.boxes, hostvecs, things, *self.thresholds)
+            results = res if results is None else results + res
         if self.mask_format == "rle":
             attach_rle(results)
         return results
@@ -149,8 +124,8 @@ class ImageSession:
         outs = m._prompts_forward(self, split, plan)
         done = torch.cuda.Event()
         done.record(torch.cuda.current_stream(m.device))
-        return PendingPrompts(m, outs, self.image_hw, self.seg_info[:1], self.boxes[:1], done, things,
-                              (m.object_mask_threshold, m.overlap_threshold), mask_format)
+        return PendingSeg(m, [(out, None, t) for out, t in zip(outs, things)], self.image_hw, self.seg_info[:1],
+                          self.boxes[:1], done, (m.object_mask_threshold, m.overlap_threshold), mask_format)
 
 
 MASK_FORMATS = ("dense", "rle")
@@ -164,6 +139,26 @@ def _content_key(t):
         return tuple(_content_key(x) for x in t)
     t = torch.as_tensor(t).detach().cpu().contiguous()
     return (tuple(t.shape), str(t.dtype), t.numpy().tobytes())
+
+
+_PLAN_TENSORS = ("tok_ids", "img_pos", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool")
+
+
+def _graph_copy(plan, names=_PLAN_TENSORS):
+    """Shallow copy of a plan (SequencePlan / PromptSplit) with its own clones of the device tensors `names`, for a CUDA
+    graph to read: the cached plan they came from may be evicted and freed.  `_graph_refresh` fills them before a replay."""
+    static = copy.copy(plan)
+    for n in names:
+        t = getattr(plan, n)
+        setattr(static, n, None if t is None else t.clone())
+    return static
+
+
+def _graph_refresh(static, plan, names=_PLAN_TENSORS):
+    for n in names:
+        t = getattr(plan, n)
+        if t is not None:
+            getattr(static, n).copy_(t, non_blocking=True)
 
 
 def attach_rle(results):
@@ -209,7 +204,7 @@ class PSALM:
         self.use_cuda_graph = use_cuda_graph
         # one fused kernel for the task heads (16-bit storage); fp32 parity runs keep the exact torch path
         self._fused_postprocess = dtype != torch.float32
-        self.overlap_branches = not os.environ.get("PSALM_NO_OVERLAP")   # pixel decoder || LLM prefill on two streams
+        self.overlap_branches = True   # pixel decoder || LLM prefill on two streams
         self.cfg, self.dtype, self.device = cfg, dtype, torch.device(device)
         sd = state_dict
         cv = lambda t: t.to(device=device, dtype=dtype).contiguous()  # noqa: E731
@@ -374,11 +369,26 @@ class PSALM:
         with self._precision_scope():
             return self._forward_core(images, plan, trace)
 
-    def _forward_core(self, images, plan, trace=None):
-        toks, sizes = self.model.vision_tower.forward_tokens(images)                 # Swin, once
+    def _swin_project(self, images):
+        """Swin (once) and the projector: (Swin token maps, their sizes, projector tokens [B,n_img,hidden])."""
+        toks, sizes = self.model.vision_tower.forward_tokens(images)
         h5, w5 = sizes[3]
-        res5 = toks[3].view(toks[3].shape[0], h5, w5, -1).permute(0, 3, 1, 2)
-        img_tok = self.model.mm_projector(res5)                                        # [B,n_img,hidden]
+        img_tok = self.model.mm_projector(toks[3].view(toks[3].shape[0], h5, w5, -1).permute(0, 3, 1, 2))
+        return toks, sizes, img_tok
+
+    def _llm_heads(self, plan, hidden):
+        """(seg queries, SEG embedding, class-name embeddings) from the LLM's hidden states; None for a head the prompt
+        has no rows for."""
+        seg_q = F.linear(SEQ.gather_seg_query(plan, hidden), *self.proj["seg_query_projector"])
+        SEG_emb = cls_emb = None
+        if plan.refer_pool is not None:
+            SEG_emb = F.linear(SEQ.pool(plan.refer_pool, hidden), *self.proj["SEG_token_projector"])
+        if plan.cls_pool is not None:
+            cls_emb = F.linear(SEQ.pool(plan.cls_pool, hidden), *self.proj["class_name_projector"])
+        return seg_q, SEG_emb, cls_emb
+
+    def _forward_core(self, images, plan, trace=None):
+        toks, sizes, img_tok = self._swin_project(images)
         # The pixel decoder needs only the Swin maps, the LLM only the projector tokens: the two branches run on two
         # streams (also inside a captured graph) and meet at the mask decoder.  The LLM branch is a chain of library GEMMs
         # at the tensor-core peak whose last waves leave SMs idle; the pixel decoder's memory-bound kernels fill them.
@@ -387,7 +397,7 @@ class PSALM:
             # (graph capture only: eager launches are host bound, two streams would buy nothing there)
             main = torch.cuda.current_stream(self.device)
             if not hasattr(self, "_branch_stream"):
-                self._branch_stream = torch.cuda.Stream(device=self.device, priority=-1 if os.environ.get("PSALM_BRANCH_PRIO") else 0)
+                self._branch_stream = torch.cuda.Stream(device=self.device)
             self._branch_stream.wait_stream(main)
             with torch.cuda.stream(self._branch_stream):
                 branch = self.pixel_decoder.forward_tokens(toks, sizes)
@@ -397,19 +407,13 @@ class PSALM:
         if plan.region_pos is not None:
             src_tok = img_tok
             if plan.vp_images is not None:   # DAVIS variant: pooled from the visual-prompt frame's map (llava_phi.py:1665-1670)
-                vtoks, vsizes = self.model.vision_tower.forward_tokens(plan.vp_images)
-                src_tok = self.model.mm_projector(vtoks[3].view(vtoks[3].shape[0], vsizes[3][0], vsizes[3][1], -1).permute(0, 3, 1, 2))
+                src_tok = self._swin_project(plan.vp_images)[2]
             region_feat = self._region_features(src_tok, plan)
         embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok, self.seg_query, region_feat)
         # (cutting the batch into groups on separate streams so that the prefill GEMMs fill each other's tail waves was
         # measured and is slower: 20.8 ms / 21.9 ms per step of 4 for 2 / 4 groups against 19.5 ms)
         hidden = self.model.phi(embeds, plan.attention_mask if plan.any_padding else None)
-        seg_q = F.linear(SEQ.gather_seg_query(plan, hidden), *self.proj["seg_query_projector"])
-        SEG_emb = cls_emb = None
-        if plan.refer_pool is not None:
-            SEG_emb = F.linear(SEQ.pool(plan.refer_pool, hidden), *self.proj["SEG_token_projector"])
-        if plan.cls_pool is not None:
-            cls_emb = F.linear(SEQ.pool(plan.cls_pool, hidden), *self.proj["class_name_projector"])
+        seg_q, SEG_emb, cls_emb = self._llm_heads(plan, hidden)
         region_emb = None
         if plan.region_pos is not None:     # llava_phi.py:1385-1388: hidden states at the <region> rows -> region_projector
             if "region_projector" not in self.proj:
@@ -433,86 +437,76 @@ class PSALM:
         return out
 
     # ---- CUDA-graph replay of the device-only part -------------------------------------------------
-    def _post_device(self, out, image_hw, geoms=None):
-        """Device part of the fused post-processing for every image (capturable); None if not applicable.
-        geoms: per image (oh, ow, height, width) = un-padded box and output size; None = no crop, output = padded size."""
-        Hi, Wi = image_hw
-        d = self.size_divisibility
-        Hp, Wp = (Hi + d - 1) // d * d, (Wi + d - 1) // d * d
-        H4, W4 = out["mask_size"]
-        B, Q = out["pred_masks"].shape[:2]
-        cls = out["pred_class_name_logits"]
-        if not (self.fused_postprocess and Hp >= 2 * H4 and Wp >= 2 * W4 and Q <= 104 and
-                (cls is None or cls.shape[-1] - 1 <= 144)):
-            return None
-        from . import kernels
-        thing = PP.thing_tensor(self.is_thing_list, self.device) if (self.panoptic_on and self.instance_on) else None
-        pm = out["pred_masks"].view(B, Q, H4, W4)
-        sizes, crops = [], []
-        for b in range(B):
-            oh, ow, height, width = geoms[b] if geoms is not None else (Hp, Wp, Hp, Wp)
-            sizes.append((height, width))
-            crops.append(None if (oh, ow, height, width) == (Hp, Wp, Hp, Wp) else (Hp, Wp, oh, ow))
-        if os.environ.get("PSALM_NO_BATCH_POST"):
-            return [PP.fused_device(kernels, pm[b], sizes[b][0], sizes[b][1], cls[b] if cls is not None else None,
-                                    out["pred_SEG_logits"][b] if out["pred_SEG_logits"] is not None else None, thing,
-                                    self.semantic_on, self.instance_on, self.panoptic_on, self.referring_on,
-                                    self.test_topk_per_image, self.object_mask_threshold, crop=crops[b]) for b in range(B)]
-        return PP.fused_device_batch(kernels, pm, sizes, cls, out["pred_SEG_logits"], thing, self.semantic_on,
-                                     self.instance_on, self.panoptic_on, self.referring_on, self.test_topk_per_image,
-                                     self.object_mask_threshold, crops=crops)
+    # Every graph table is a bounded LRU: each entry owns static buffers + a private pool (hundreds of MB at 1024^2, B = 4)
+    MAX_GRAPHS = 8
+    MAX_PLANS = 16
 
-    MAX_GRAPHS = 8   # each entry owns static buffers + a private pool (hundreds of MB at 1024^2, B = 4)
+    def _lru(self, table, key, make, bound):
+        """The entry of `key` in the bounded LRU cache `self.<table>`, made by `make()` on a miss; when the table is
+        full the least recently used entry goes."""
+        cache = self.__dict__.setdefault(table, OrderedDict())
+        ent = cache.get(key)
+        if ent is None:
+            ent = make()
+            while len(cache) >= bound:
+                cache.popitem(last=False)
+            cache[key] = ent
+        cache.move_to_end(key)
+        return ent
 
+    def _capture(self, fn):
+        """(CUDA graph of fn(), its output): two warm-up calls on a side stream, then the capture."""
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(side), self._precision_scope():
+            for _ in range(2):
+                fn()
+        torch.cuda.current_stream(self.device).wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        g = torch.cuda.CUDAGraph()
+        with self._precision_scope(), torch.cuda.graph(g):
+            out = fn()
+        return g, out
+
+    def _forward_post(self, images, plan, geoms):
+        """forward_core, plus the device part of the fused task heads for the per-image geometries `geoms` when every
+        image takes the fused kernel (capturable)."""
+        out = self._forward_core(images, plan)
+        if geoms is not None:
+            hw = tuple(images.shape[-2:])
+            routes = self._routes(hw, geoms, out)
+            if all(r is not None for r in routes):
+                out["post"] = self._post_device(out, hw, routes, getattr(self, "is_thing_list", None),
+                                                self.object_mask_threshold)
+                out["post_geoms"] = geoms
+        return out
+
+    @torch.no_grad()
     def forward_core_graphed(self, images, plan, lane=0, fuse_post=True):
-        # fuse_post: True (no crop / resize), False (task heads outside the graph) or a tuple of per-image geometries
         """Same results as forward_core, replayed from a CUDA graph captured per (image size, prompt
         structure): the ~800 launches of one image become one graph launch (the reference issues them
         one by one from Python, plus ~150 extra tiny launches in its decoder).  `lane` selects an
-        independent graph + static buffers so that several images can be in flight on different streams."""
-        geoms = fuse_post if isinstance(fuse_post, tuple) else None
+        independent graph + static buffers so that several images can be in flight on different streams.
+        `fuse_post` (`_fused_applies`): True (no crop / resize) or a tuple of per-image geometries puts the device part
+        of the fused task heads into the graph; False leaves the task heads to `post_process`."""
         key = (lane, fuse_post, self.seg_task, float(self.object_mask_threshold), tuple(getattr(self, "is_thing_list", None) or ()), tuple(images.shape), str(images.dtype), plan.B,
                plan.T, plan.n_img, plan.any_padding,
                None if plan.cls_pool is None else tuple(plan.cls_pool.shape), plan.refer_pool is not None,
                None if plan.pad_pos is None else int(plan.pad_pos.numel()))
-        if not hasattr(self, "_graphs"):
-            self._graphs = OrderedDict()
-        ent = self._graphs.get(key)
-        if ent is not None:
-            self._graphs.move_to_end(key)
-        tensors = ("tok_ids", "img_pos", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool")
-        if ent is None:
-            import copy
-            static_img = images.clone()
-            static_plan = copy.copy(plan)
-            for n in tensors:
-                t = getattr(plan, n)
-                setattr(static_plan, n, None if t is None else t.clone())
-            side = torch.cuda.Stream(device=self.device)
-            side.wait_stream(torch.cuda.current_stream(self.device))
-            hw = tuple(images.shape[-2:])
-            with torch.cuda.stream(side):
-                for _ in range(2):
-                    o = self.forward_core(static_img, static_plan)
-                    o["post"] = self._post_device(o, hw, geoms) if fuse_post else None
-            torch.cuda.current_stream(self.device).wait_stream(side)
-            torch.cuda.synchronize(self.device)
-            g = torch.cuda.CUDAGraph()
-            with self._precision_scope(), torch.cuda.graph(g):
-                static_out = self._forward_core(static_img, static_plan)
-                # task heads' device part in the same graph (only when every image takes the fused path)
-                static_out["post"] = self._post_device(static_out, hw, geoms) if fuse_post else None
-                static_out["post_geoms"] = geoms
-            ent = (g, static_img, static_plan, static_out)
-            while len(self._graphs) >= self.MAX_GRAPHS:   # least recently used graph and its static buffers go
-                self._graphs.popitem(last=False)
-            self._graphs[key] = ent
-        g, static_img, static_plan, static_out = ent
+        geoms = None
+        if isinstance(fuse_post, tuple):
+            geoms = fuse_post
+        elif fuse_post:
+            Hp, Wp = self._padded(images.shape[-2:])
+            geoms = ((Hp, Wp, Hp, Wp),) * images.shape[0]      # no crop / resize
+
+        def make():
+            static_img, static_plan = images.clone(), _graph_copy(plan)
+            g, static_out = self._capture(lambda: self._forward_post(static_img, static_plan, geoms))
+            return g, static_img, static_plan, static_out
+        g, static_img, static_plan, static_out = self._lru("_graphs", key, make, self.MAX_GRAPHS)
         static_img.copy_(images, non_blocking=True)
-        for n in tensors:
-            t = getattr(plan, n)
-            if t is not None:
-                getattr(static_plan, n).copy_(t, non_blocking=True)
+        _graph_refresh(static_plan, plan)
         g.replay()
         return static_out
 
@@ -546,9 +540,7 @@ class PSALM:
 
     def _image_core(self, images):
         """Prompt-independent device work of one image (capturable)."""
-        toks, sizes = self.model.vision_tower.forward_tokens(images)
-        h5, w5 = sizes[3]
-        img_tok = self.model.mm_projector(toks[3].view(toks[3].shape[0], h5, w5, -1).permute(0, 3, 1, 2))
+        toks, sizes, img_tok = self._swin_project(images)
         mask_features, ms, ms_sizes = self.pixel_decoder.forward_tokens(toks, sizes)
         mem = self.predictor.memory(ms, ms_sizes, mask_features, sizes[0], self.num_queries)
         return dict(swin=toks, swin_sizes=sizes, img_tok=img_tok, mask_features=mask_features, ms=ms, ms_sizes=ms_sizes,
@@ -576,12 +568,7 @@ class PSALM:
             img_tok = state["img_tok"]
             embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok[:, :0], self.seg_query)
             hidden = self.model.phi.forward_suffix(embeds, cache, plan.attention_mask if plan.any_padding else None)
-            seg_q = F.linear(SEQ.gather_seg_query(plan, hidden), *self.proj["seg_query_projector"])
-            SEG_emb = cls_emb = None
-            if plan.refer_pool is not None:
-                SEG_emb = F.linear(SEQ.pool(plan.refer_pool, hidden), *self.proj["SEG_token_projector"])
-            if plan.cls_pool is not None:
-                cls_emb = F.linear(SEQ.pool(plan.cls_pool, hidden), *self.proj["class_name_projector"])
+            seg_q, SEG_emb, cls_emb = self._llm_heads(plan, hidden)
             out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
                                                 memory=state["mem"])
             out["mask_size"] = state["mask_size"]
@@ -591,21 +578,15 @@ class PSALM:
     def _cached_split(self, prompts, image_hw):
         """(host PromptSplit, device suffix plan) of a prompt set, cached by content like `_cached_plan`."""
         key = (tuple(image_hw),) + tuple(tuple(_content_key(p.get(n)) for n in SEQ.PROMPT_KEYS) for p in prompts)
-        if not hasattr(self, "_splits"):
-            self._splits = OrderedDict()
-        ent = self._splits.get(key)
-        if ent is None:
+
+        def make():
             import dataclasses
             split = SEQ.split_prompts(prompts, self.make_plan_n_img(image_hw), self.num_queries)
             plan = split.suffix.to(self.device)
             split = dataclasses.replace(split, tok_ids=split.tok_ids.to(self.device), img_pos=split.img_pos.to(self.device),
                                         suffix=None)
-            ent = (split, plan)
-            while len(self._splits) >= 16:
-                self._splits.popitem(last=False)
-            self._splits[key] = ent
-        self._splits.move_to_end(key)
-        return ent
+            return split, plan
+        return self._lru("_splits", key, make, self.MAX_PLANS)
 
     def make_plan_n_img(self, image_hw):
         """Projector tokens of an image of size image_hw (the <image> expansion of make_plan)."""
@@ -619,33 +600,7 @@ class PSALM:
     # CUDA graphs of the session phases: the image (per lane, image shape and dtype), the prefix prefill (per lane, image
     # key and prefix content) and the prompt pass (per lane, prefix, K, suffix length and plan structure, task heads).
     # Later phases read the static buffers of the earlier ones of the same lane, so a session is valid until the next
-    # open_image on its lane.  Bounded LRUs like MAX_GRAPHS.
-    MAX_SESSION_GRAPHS = 8
-
-    def _capture(self, fn):
-        side = torch.cuda.Stream(device=self.device)
-        side.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(side), self._precision_scope():
-            for _ in range(2):
-                fn()
-        torch.cuda.current_stream(self.device).wait_stream(side)
-        torch.cuda.synchronize(self.device)
-        g = torch.cuda.CUDAGraph()
-        with self._precision_scope(), torch.cuda.graph(g):
-            out = fn()
-        return g, out
-
-    def _session_graph(self, table, key, make):
-        graphs = self.__dict__.setdefault(table, OrderedDict())
-        ent = graphs.get(key)
-        if ent is None:
-            ent = make()
-            while len(graphs) >= self.MAX_SESSION_GRAPHS:
-                graphs.popitem(last=False)
-            graphs[key] = ent
-        graphs.move_to_end(key)
-        return ent
-
+    # open_image on its lane.
     def _image_graphed(self, images, lane):
         key = (lane, tuple(images.shape), str(images.dtype))
 
@@ -653,10 +608,12 @@ class PSALM:
             static_img = images.clone()
             g, state = self._capture(lambda: self._image_core(static_img))
             return g, static_img, state
-        g, static_img, state = self._session_graph("_image_graphs", key, make)
+        g, static_img, state = self._lru("_image_graphs", key, make, self.MAX_GRAPHS)
         static_img.copy_(images, non_blocking=True)
         g.replay()
         return state
+
+    _PREFIX_TENSORS = ("tok_ids", "img_pos")
 
     def _prefix_for(self, sess, split):
         if not self.use_cuda_graph:
@@ -665,24 +622,18 @@ class PSALM:
         key = (sess.lane, id(sess.state), split.prefix_ids.tobytes())
 
         def make():
-            import dataclasses
             from .generate import PagedKVCache
             page = -(-split.P // 64) * 64
             cache = PagedKVCache(self.cfg.phi, 1, page, self.dtype, self.device, page_size=page)
-            # the graph reads its own copies of the prefix rows' token ids and image rows (the split that brought them
-            # lives in a bounded cache and may be freed); they are refreshed before every replay
-            static = dataclasses.replace(split, tok_ids=split.tok_ids.clone(), img_pos=split.img_pos.clone())
+            static = _graph_copy(split, self._PREFIX_TENSORS)
             g, _ = self._capture(lambda: self._prefix_core(sess.state, static, cache))
             # the replayed writes start at seq_lens (0): only the host-side length moves (forward_suffix reads it)
             cache.length = split.P
             return g, cache, sess.state, static
-        g, cache, _, static = self._session_graph("_prefix_graphs", key, make)
-        static.tok_ids.copy_(split.tok_ids, non_blocking=True)
-        static.img_pos.copy_(split.img_pos, non_blocking=True)
+        g, cache, _, static = self._lru("_prefix_graphs", key, make, self.MAX_GRAPHS)
+        _graph_refresh(static, split, self._PREFIX_TENSORS)
         g.replay()
         return cache
-
-    _PLAN_TENSORS = ("tok_ids", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool")
 
     def _prompts_graphed(self, sess, cache, split, plan):
         key = (sess.lane, id(sess.state), id(cache), plan.B, plan.T, plan.any_padding,
@@ -690,18 +641,11 @@ class PSALM:
                None if plan.pad_pos is None else int(plan.pad_pos.numel()), self.seg_task)
 
         def make():
-            import copy
-            static_plan = copy.copy(plan)
-            for n in self._PLAN_TENSORS:
-                t = getattr(plan, n)
-                setattr(static_plan, n, None if t is None else t.clone())
+            static_plan = _graph_copy(plan)
             g, out = self._capture(lambda: self._prompts_core(sess.state, cache, static_plan))
             return g, static_plan, out, (sess.state, cache)
-        g, static_plan, out, _ = self._session_graph("_prompt_graphs", key, make)
-        for n in self._PLAN_TENSORS:
-            t = getattr(plan, n)
-            if t is not None:
-                getattr(static_plan, n).copy_(t, non_blocking=True)
+        g, static_plan, out, _ = self._lru("_prompt_graphs", key, make, self.MAX_GRAPHS)
+        _graph_refresh(static_plan, plan)
         g.replay()
         return out
 
@@ -755,16 +699,9 @@ class PSALM:
         key = (tuple(image_hw),) + tuple(_content_key(t) for t in (input_ids, attention_mask, class_name_ids, cls_indices,
                                                               class_name_embedding_indices, token_refer_id,
                                                               refer_embedding_indices))
-        if not hasattr(self, "_plans"):
-            self._plans = {}
-        plan = self._plans.get(key)
-        if plan is None:
-            if len(self._plans) >= 16:
-                self._plans.pop(next(iter(self._plans)))
-            plan = self.make_plan(input_ids, attention_mask, image_hw, class_name_ids, cls_indices,
-                                  class_name_embedding_indices, token_refer_id, refer_embedding_indices).to(self.device)
-            self._plans[key] = plan
-        return plan
+        return self._lru("_plans", key, lambda: self.make_plan(
+            input_ids, attention_mask, image_hw, class_name_ids, cls_indices, class_name_embedding_indices, token_refer_id,
+            refer_embedding_indices).to(self.device), self.MAX_PLANS)
 
     @torch.no_grad()
     def eval_seg(self, input_ids=None, attention_mask=None, past_key_values=None, inputs_embeds=None, labels=None,
@@ -811,7 +748,6 @@ class PSALM:
                                  class_name_embedding_indices, token_refer_id, refer_embedding_indices)
         has_regions = plan.region_pos is not None
         if has_regions:   # llava_phi.py:1346-1349: the regions come with the request (seg_info[i]['instances'].region_masks)
-            import copy
             from .region import region_inputs
             pts, img, counts = region_inputs(seg_info, region_points, "region_masks" if vp_images is None else "vp_region_masks")
             assert counts == plan.region_counts, "the munber of <region> tokens and regions needs to be same"   # llava_phi.py:593
@@ -846,78 +782,106 @@ class PSALM:
                 hostvecs.append(pin)
         done = torch.cuda.Event()
         done.record(cur)
-        return PendingSeg(self, out, tuple(images.shape[-2:]), seg_info, boxes, done, hostvecs,
-                          getattr(self, "is_thing_list", None), (self.object_mask_threshold, self.overlap_threshold),
-                          mask_format)
+        return PendingSeg(self, [(out, hostvecs, getattr(self, "is_thing_list", None))], tuple(images.shape[-2:]), seg_info,
+                          boxes, done, (self.object_mask_threshold, self.overlap_threshold), mask_format)
+
+    def _padded(self, image_hw):
+        """Size of the padded batch (ImageList.from_tensors(images, 32), llava_phi.py:1400)."""
+        d = self.size_divisibility
+        return tuple((x + d - 1) // d * d for x in image_hw)
+
+    def _geoms(self, image_hw, seg_info, boxes):
+        """Per image (oh, ow, height, width): the un-padded box and the output size."""
+        return tuple((box[0], box[1], info.get("height", image_hw[0]), info.get("width", image_hw[1]))
+                     for info, box in zip(seg_info, boxes))
+
+    def _routes(self, image_hw, geoms, out=None):
+        """Which task heads serve each image: its geometry (`_geoms`) when the fused kernel does - the composed
+        up-sample -> crop -> resize unless the geometry is the padded size itself -, None for the torch heads.  `out`:
+        forward_core's output; None before the forward, when the class count is not known yet (decided again on `out`)."""
+        Hp, Wp = self._padded(image_hw)
+        if out is None:
+            ps = self.cfg.swin.patch
+            Q, ncls, (H4, W4) = self.num_queries, 0, (-(-image_hw[0] // ps), -(-image_hw[1] // ps))
+        else:
+            cls = out["pred_class_name_logits"]
+            Q, ncls, (H4, W4) = out["pred_masks"].shape[1], 0 if cls is None else cls.shape[-1] - 1, out["mask_size"]
+        if not (self.fused_postprocess and Q <= PP.FUSED_MAX_QUERIES and ncls <= PP.FUSED_MAX_CLASSES and
+                Hp >= 2 * H4 and Wp >= 2 * W4):
+            return [None] * len(geoms)
+        from . import kernels
+        return [g if g == (Hp, Wp, Hp, Wp) or (self.sem_seg_postprocess_before_inference and kernels.postproc_crop_supported(
+                    Q, H4, W4, Hp, Wp, *g, PP.FUSED_MAX_CLASSES)) else None
+                for g in geoms]
+
+    def _post_device(self, out, image_hw, routes, is_thing_list, obj_thr):
+        """Device part of the fused task heads (capturable) for the images `routes` sends to the fused kernel: per image
+        the dict `PP.fused_host` finishes, None for the images of the torch heads."""
+        idx = [b for b, r in enumerate(routes) if r is not None]
+        post = [None] * len(routes)
+        if not idx:
+            return post
+        from . import kernels
+        Hp, Wp = self._padded(image_hw)
+        H4, W4 = out["mask_size"]
+        B, Q = out["pred_masks"].shape[:2]
+        pick = lambda t: t if t is None or len(idx) == B else t[idx]   # noqa: E731
+        thing = PP.thing_tensor(is_thing_list, self.device) if (self.panoptic_on and self.instance_on) else None
+        ds = PP.fused_device_batch(kernels, pick(out["pred_masks"]).view(len(idx), Q, H4, W4), [routes[b][2:] for b in idx],
+                                   pick(out["pred_class_name_logits"]), pick(out["pred_SEG_logits"]), thing,
+                                   self.semantic_on, self.instance_on, self.panoptic_on, self.referring_on,
+                                   self.test_topk_per_image, obj_thr,
+                                   crops=[None if routes[b] == (Hp, Wp, Hp, Wp) else (Hp, Wp) + routes[b][:2] for b in idx])
+        for b, d in zip(idx, ds):
+            post[b] = d
+        return post
 
     def _fused_applies(self, image_hw, seg_info):
         """(fuse_post, boxes): fuse_post is True when every image takes the fused task-head kernel without crop / resize,
         a tuple of per-image (oh, ow, height, width) when the composed up-sample -> crop -> resize kernel applies to all of
         them (the reference's mapper flow: padded 1024^2 input, original-size output), False otherwise (the graph is then
         captured without the task heads instead of running them for nothing)."""
-        Hi, Wi = image_hw
-        d = self.size_divisibility
-        Hp, Wp = (Hi + d - 1) // d * d, (Wi + d - 1) // d * d
         boxes = [PP.unpadded_box(info["padding_mask"]) for info in seg_info]
-        geoms = tuple((box[0], box[1], info.get("height", Hi), info.get("width", Wi)) for info, box in zip(seg_info, boxes))
+        geoms = self._geoms(image_hw, seg_info, boxes)
+        Hp, Wp = self._padded(image_hw)
         if all(g == (Hp, Wp, Hp, Wp) for g in geoms):
             return True, boxes
-        if not (self.fused_postprocess and self.sem_seg_postprocess_before_inference):
-            return False, boxes
-        from . import kernels
-        ps = self.cfg.swin.patch
-        H4, W4 = -(-Hi // ps), -(-Wi // ps)
-        ncls = 144
-        ok = all(kernels.postproc_crop_supported(self.num_queries, H4, W4, Hp, Wp, g[0], g[1], g[2], g[3], ncls) or
-                 g == (Hp, Wp, Hp, Wp) for g in geoms) and self.num_queries <= 104 and Hp >= 2 * H4 and Wp >= 2 * W4
-        return (geoms if ok else False), boxes
+        return (geoms if all(r is not None for r in self._routes(image_hw, geoms)) else False), boxes
 
     @torch.no_grad()
-    def post_process(self, out, image_hw, seg_info, boxes=None, hostvecs=None):
+    def post_process(self, out, image_hw, seg_info, boxes=None, hostvecs=None, is_thing_list=None,
+                     object_mask_threshold=None, overlap_threshold=None):
         """llava_phi.py:1395-1472 for EVERY image of the batch.  `boxes`: un-padded (h, w) per image when the
         caller already derived them from the padding masks; `hostvecs`: the fused heads' host vectors when they were
-        already copied to (pinned) host memory."""
+        already copied to (pinned) host memory.  `is_thing_list` and the panoptic thresholds default to the model's
+        attributes.  The fused heads' device part runs here unless `out` already holds it for these geometries."""
+        if is_thing_list is None:
+            is_thing_list = getattr(self, "is_thing_list", None)
+        obj_thr = self.object_mask_threshold if object_mask_threshold is None else object_mask_threshold
+        ovl_thr = self.overlap_threshold if overlap_threshold is None else overlap_threshold
         with self._precision_scope():
-            return self._post_process(out, image_hw, seg_info, boxes, hostvecs)
+            return self._post_process(out, image_hw, seg_info, boxes, hostvecs, is_thing_list, obj_thr, ovl_thr)
 
-    def _post_process(self, out, image_hw, seg_info, boxes=None, hostvecs=None):
-        Hi, Wi = image_hw
-        d = self.size_divisibility
-        Hp, Wp = (Hi + d - 1) // d * d, (Wi + d - 1) // d * d     # ImageList.from_tensors(images, 32), :1400
+    def _post_process(self, out, image_hw, seg_info, boxes, hostvecs, is_thing_list, obj_thr, ovl_thr):
+        Hp, Wp = self._padded(image_hw)
         H4, W4 = out["mask_size"]
         B, Q = out["pred_masks"].shape[:2]
+        if boxes is None:
+            boxes = [PP.unpadded_box(info["padding_mask"]) for info in seg_info]
+        geoms = self._geoms(image_hw, seg_info, boxes)
+        post = out.get("post")
+        if post is None or out["post_geoms"] != geoms:
+            post, hostvecs = self._post_device(out, image_hw, self._routes(image_hw, geoms, out), is_thing_list, obj_thr), None
         pm = out["pred_masks"].view(B, Q, H4, W4)
         mask_pred = None
         results = []
         for b in range(B):
-            info = seg_info[b]
-            height, width = info.get("height", Hi), info.get("width", Wi)
-            oh, ow = boxes[b] if boxes is not None else PP.unpadded_box(info["padding_mask"])
-            cls_b = out["pred_class_name_logits"][b] if out["pred_class_name_logits"] is not None else None
-            seg_b = out["pred_SEG_logits"][b] if out["pred_SEG_logits"] is not None else None
-            trivial = (oh, ow) == (Hp, Wp) and (height, width) == (Hp, Wp)
-            pg = out.get("post_geoms")
-            if out.get("post") is not None and ((pg is None and trivial) or (pg is not None and pg[b] == (oh, ow, height, width))):
-                results.append(PP.fused_host(out["post"][b], getattr(self, "is_thing_list", None), self.overlap_threshold,
+            if post[b] is not None:
+                results.append(PP.fused_host(post[b], is_thing_list, ovl_thr,
                                              host=None if hostvecs is None or hostvecs[b] is None else hostvecs[b].numpy()))
                 continue
-            if (not trivial and self.fused_postprocess and self.sem_seg_postprocess_before_inference and Q <= 104 and
-                    Hp >= 2 * H4 and Wp >= 2 * W4 and (cls_b is None or cls_b.shape[-1] - 1 <= 144)):
-                from . import kernels
-                if kernels.postproc_crop_supported(Q, H4, W4, Hp, Wp, oh, ow, height, width, 144):
-                    results.append(PP.fused_postprocess(
-                        kernels, pm[b], height, width, cls_b, seg_b, getattr(self, "is_thing_list", None), self.semantic_on,
-                        self.instance_on, self.panoptic_on, self.referring_on, self.test_topk_per_image,
-                        self.object_mask_threshold, self.overlap_threshold, crop=(Hp, Wp, oh, ow)))
-                    continue
-            if self.fused_postprocess and trivial and Hp >= 2 * H4 and Wp >= 2 * W4 and Q <= 104 and \
-                    (cls_b is None or cls_b.shape[-1] - 1 <= 144):
-                from . import kernels
-                results.append(PP.fused_postprocess(
-                    kernels, pm[b], Hp, Wp, cls_b, seg_b, getattr(self, "is_thing_list", None), self.semantic_on,
-                    self.instance_on, self.panoptic_on, self.referring_on, self.test_topk_per_image,
-                    self.object_mask_threshold, self.overlap_threshold))
-                continue
+            info = seg_info[b]
+            oh, ow, height, width = geoms[b]
             if mask_pred is None:
                 mask_pred = F.interpolate(pm.float(), size=(Hp, Wp), mode="bilinear", align_corners=False)
             mp = mask_pred[b]
@@ -934,12 +898,10 @@ class PSALM:
                     sem = PP.sem_seg_postprocess(sem, (oh, ow), height, width)
                 r["sem_seg"] = sem
             if self.instance_on:
-                r["instances"] = PP.instance_inference(cls, mp, self.test_topk_per_image,
-                                                       getattr(self, "is_thing_list", None), self.panoptic_on, sig)
+                r["instances"] = PP.instance_inference(cls, mp, self.test_topk_per_image, is_thing_list, self.panoptic_on,
+                                                       sig)
             if self.panoptic_on:
-                r["panoptic_seg"] = PP.panoptic_inference(cls, mp, self.is_thing_list,
-                                                          self.object_mask_threshold,
-                                                          self.overlap_threshold, sig)
+                r["panoptic_seg"] = PP.panoptic_inference(cls, mp, is_thing_list, obj_thr, ovl_thr, sig)
             if self.referring_on:
                 r["instances"] = PP.seg_instance_inference(out["pred_SEG_logits"][b].float(), mp,
                                                            self.test_topk_per_image, sig)

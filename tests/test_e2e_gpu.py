@@ -262,7 +262,7 @@ def test_baseline_configs_full_size_bf16(task, H, W, ncls, batch):
             assert set(np.unique(pan.cpu().numpy()).tolist()) <= set([0] + [d["id"] for d in info])
 
 
-def test_mapper_flow_uses_the_fused_kernel_and_matches_the_oracle(monkeypatch):
+def test_mapper_flow_runs_the_composed_kernel_for_every_image_and_matches_the_oracle(monkeypatch):
     """The reference's real eval flow (coco_panoptic_mapper.py:148-162): image resized + padded to a square with a
     padding mask, outputs at the ORIGINAL size.  16-bit runs take the composed fused kernel (eager and CUDA graph), whose
     results must equal the step-by-step torch path on the same mask logits and track the fp32 oracle."""
@@ -274,17 +274,11 @@ def test_mapper_flow_uses_the_fused_kernel_and_matches_the_oracle(monkeypatch):
     pm[192:, :] = True                       # a 4:3 image resized to 256 x 192, padded at the bottom
     inp["seg_info"] = [dict(padding_mask=pm, height=120, width=160), dict(padding_mask=pm.clone(), height=300, width=400)]
     ores, it = _oracle(sd, inp, "panoptic")
-    calls = []
-    real = PP.fused_device
-
-    def spy(*a, **k):
-        calls.append(k.get("crop"))
-        return real(*a, **k)
-    monkeypatch.setattr(PP, "fused_device", spy)
+    calls = {False: [], True: []}        # per run: the crops of every fused_device_batch call
     real_b = PP.fused_device_batch
 
-    def spy_b(*a, **k):        # the graph path batches the small algebra of all images
-        calls.extend(k.get("crops"))
+    def spy_b(*a, **k):
+        calls[graph].append(k.get("crops"))
         return real_b(*a, **k)
     monkeypatch.setattr(PP, "fused_device_batch", spy_b)
     outs = {}
@@ -299,7 +293,8 @@ def test_mapper_flow_uses_the_fused_kernel_and_matches_the_oracle(monkeypatch):
             assert res[b]["instances"].pred_masks.shape[1:] == (hh, ww)
             a, o = res[b]["sem_seg"].float().cpu(), ores[b]["sem_seg"]
             assert (a - o).norm() / o.norm() < 0.2
-    assert calls and all(c == (256, 256, 192, 256) for c in calls)          # the composed kernel ran, never the slow path
+    for graph in (False, True):     # the composed kernel ran for every image, eager and graph, never the slow path
+        assert calls[graph] and all(c == [(256, 256, 192, 256)] * 2 for c in calls[graph]), (graph, calls[graph])
     for b in range(2):                                                       # graph replay == eager
         assert torch.equal(outs[False][b]["panoptic_seg"][0], outs[True][b]["panoptic_seg"][0])
         assert torch.equal(outs[False][b]["sem_seg"], outs[True][b]["sem_seg"])

@@ -34,6 +34,16 @@ def _reference_path(logits, cls, seg, thing, H, W, task):
     return r
 
 
+def _fused(kernels, logits, cls, seg, thing, H, W, task):
+    """The fused task heads of one image: fused_device_batch on a batch of one, then fused_host."""
+    (d,) = PP.fused_device_batch(kernels, logits[None], [(H, W)], None if task == "referring" else cls[None],
+                                 seg[None] if task == "referring" else None,
+                                 PP.thing_tensor(thing, logits.device) if task == "panoptic" else None,
+                                 task in ("semantic", "panoptic"), task in ("instance", "panoptic"), task == "panoptic",
+                                 task == "referring", 100, 0.8)
+    return PP.fused_host(d, thing, 0.8)
+
+
 def _compare(ref, got, task, sem_tol):
     if "sem_seg" in ref:
         err = (got["sem_seg"].float().cpu() - ref["sem_seg"].cpu()).abs().max() / ref["sem_seg"].abs().max()
@@ -57,15 +67,13 @@ def _compare(ref, got, task, sem_tol):
 
 
 @pytest.mark.parametrize("task", ["panoptic", "instance", "semantic", "referring"])
-def test_fused_glue_cpu(monkeypatch, task):
+def test_fused_heads_batch_of_one_cpu(monkeypatch, task):
     from psalm_b200 import kernels
     monkeypatch.setattr(kernels, "postproc_fused", emu.postproc_fused)
     logits, cls, seg, thing = _inputs(3)
     H, W = 96, 160
     ref = _reference_path(logits, cls, seg, thing, H, W, task)
-    got = PP.fused_postprocess(kernels, logits, H, W, None if task == "referring" else cls, seg if task == "referring" else None,
-                               thing, task in ("semantic", "panoptic"), task in ("instance", "panoptic"),
-                               task == "panoptic", task == "referring")
+    got = _fused(kernels, logits, cls, seg, thing, H, W, task)
     _compare(ref, got, task, 2e-3)
 
 
@@ -95,14 +103,12 @@ def test_batched_glue_cpu(monkeypatch, task):
 @pytest.mark.parametrize("task", ["panoptic", "instance", "semantic", "referring"])
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16, torch.float32])
 @pytest.mark.parametrize("shape", [(24, 40, 96, 160), (50, 66, 200, 264), (13, 21, 61, 85)])
-def test_fused_kernel_gpu(task, dt, shape):
+def test_fused_heads_batch_of_one_gpu(task, dt, shape):
     from psalm_b200 import kernels
     H4, W4, H, W = shape
     logits, cls, seg, thing = _inputs(5, H4=H4, W4=W4, dtype=dt)
     ref = _reference_path(logits.float(), cls, seg, thing, H, W, task)
-    got = PP.fused_postprocess(kernels, logits.cuda(), H, W, None if task == "referring" else cls.cuda(),
-                               seg.cuda() if task == "referring" else None, thing, task in ("semantic", "panoptic"),
-                               task in ("instance", "panoptic"), task == "panoptic", task == "referring")
+    got = _fused(kernels, logits.cuda(), cls.cuda(), seg.cuda(), thing, H, W, task)
     _compare(ref, got, task, 3e-3)
 
 

@@ -147,12 +147,12 @@ class _Done:
 
 class _Model:
     device = "cpu"
-    object_mask_threshold = overlap_threshold = 0.8
 
     def __init__(self, results):
         self.results = results
 
-    def post_process(self, out, image_hw, seg_info, boxes, hostvecs=None):
+    def post_process(self, out, image_hw, seg_info, boxes=None, hostvecs=None, is_thing_list=None,
+                     object_mask_threshold=None, overlap_threshold=None):
         return self.results
 
 
@@ -171,10 +171,10 @@ def _results():
 
 
 def _pending(results, mask_format):
-    return P.PendingSeg(_Model(results), None, (6, 5), None, None, _Done(), None, None, (0.8, 0.8), mask_format)
+    return P.PendingSeg(_Model(results), [(None, None, None)], (6, 5), None, None, _Done(), (0.8, 0.8), mask_format)
 
 
-def test_mask_format_dense_and_rle(monkeypatch):
+def test_pending_seg_mask_format_dense_and_rle(monkeypatch):
     monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: _Stream())
     calls = []
     monkeypatch.setattr(rle, "encode_device", lambda m: calls.append(len(m)) or _oracle_encode_device(m))
