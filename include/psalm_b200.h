@@ -343,6 +343,35 @@ int psalm_rle_strings(const uint32_t* ends, const int64_t* run_off, const int64_
 int psalm_rle_decode(const uint8_t* chars, const int64_t* byte_off, uint32_t* ends, int64_t* nruns, uint8_t* out, int n,
                      int H, int W, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Video object segmentation: the per-frame loop of eval_davis.py (psalm/eval/eval_davis.py:388-480) on the device
+ * (csrc/vos.cu).  K <= 32 objects per clip.
+ * psalm_vos_pick (eval_davis.py:443-453, scores of region_inference llava_phi.py:387-400): region_logits [K,Q] (dtype),
+ *   stats [Q,5] fp32 = summed partials of psalm_postproc_fused* (column 0 count(x>0), column 1 sum(sigmoid*[x>0])).
+ *   scores[k,q] = sigmoid(region_logits[k,q]) * stats[q,1] / (stats[q,0] + 1e-6); per object in order, the top 10
+ *   queries by score (ties: lower query first) are tried and the first one no earlier object took is picked; when all
+ *   10 are taken the object keeps the previous object's pick and score (the reference's loop variables).
+ *   pick [K] int32, score [K] fp32.  10 <= Q <= 128.  One warp.
+ * psalm_vos_fuse (fuse_davis_mask eval_davis.py:337-342, the IoU counts of :463-473, detectron2
+ *   ResizeTransform.apply_segmentation (Pillow NEAREST) + FixedSizeCrop zero padding of the kept masks, :406-408):
+ *   masks [K,H,W] fp32 (non-zero = set) at the output size.  labels [H,W] uint8 = fill[k] of the last object set at
+ *   the pixel, 0 elsewhere; area [K] int32; inter [K,K] int32 = pixels set in both.  labels may be null: then only the
+ *   bits are written (area / inter are then unused).  bits [K,Hp,ceil(Wp/32)] uint32: bit x of row y of mask k =
+ *   masks[k, src_row[y], src_col[x]] != 0, 0 where src_row[y] or src_col[x] is -1 (the padding and Pillow's
+ *   out-of-range taps; the tables restate Pillow's ImagingScaleAffine index arithmetic, computed by the caller).
+ *   row_prefix [K,Hp+1] int32 = exclusive prefix sum of the set pixels per row, count [K] int32 = set pixels.
+ * psalm_region_points_gather (region.py sample_region_points = context_cluster.py:31-40, :349-352): for region r and
+ *   point p, the sel[r,p]-th set pixel (row-major, the order of nonzero()) of mask mask_of_region[r] of bits /
+ *   row_prefix (layout of psalm_vos_fuse, M masks) -> points [R,P,2] fp32 = (y / Hp, x / Wp), IEEE divisions.  The
+ *   caller draws sel on the host with the reference's randint / randperm calls. */
+int psalm_vos_pick(const void* region_logits, const float* stats, int* pick, float* score, int K, int Q, int dtype,
+                   void* stream);
+int psalm_vos_fuse(const float* masks, const int* fill, const int* src_row, const int* src_col, uint8_t* labels,
+                   int* area, int* inter, uint32_t* bits, int* row_prefix, int* count, int K, int H, int W, int Hp, int Wp,
+                   void* stream);
+int psalm_region_points_gather(const uint32_t* bits, const int* row_prefix, const int* sel, const int* mask_of_region,
+                               float* points, int R, int P, int Hp, int Wp, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

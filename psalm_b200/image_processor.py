@@ -79,6 +79,33 @@ def pil_bilinear_resize(image_hwc_u8, out_h, out_w):
     return x.to(torch.uint8)
 
 
+def pil_nearest_index(in_size, out_size):
+    """int64 [out_size]: the source index of every output column (or row) of `PIL.Image.resize(..., Image.NEAREST)`, -1
+    where Pillow leaves the pixel unset (0).  Pillow's ImagingScaleAffine (Geometry.c) starts at scale / 2 and ADDS the
+    scale (in double) once per output pixel, truncating each sum; evaluating (x + 0.5) * scale directly instead differs
+    from Pillow at some sizes (tests/test_video_cpu.py compares both axes with Pillow)."""
+    scale = in_size / out_size
+    idx = np.empty(out_size, dtype=np.int64)
+    xo = scale * 0.5
+    for x in range(out_size):
+        xin = -1 if xo < 0.0 else int(xo)
+        idx[x] = xin if xin < in_size else -1
+        xo += scale
+    return idx
+
+
+def nearest_pad_tables(height, width, resized_hw, padded_hw):
+    """detectron2 `ResizeTransform.apply_segmentation` (Pillow NEAREST from (height, width) to `resized_hw`) followed by
+    FixedSizeCrop's zero padding to `padded_hw` (seg_pad_value=0, coco_*_mapper.py build_transform_gen), as source-row
+    and source-column tables: int32 [Hp] and [Wp], -1 = zero."""
+    (oh, ow), (Hp, Wp) = resized_hw, padded_hw
+    rows = np.full(Hp, -1, dtype=np.int32)
+    cols = np.full(Wp, -1, dtype=np.int32)
+    rows[:oh] = pil_nearest_index(height, oh)
+    cols[:ow] = pil_nearest_index(width, ow)
+    return torch.from_numpy(rows), torch.from_numpy(cols)
+
+
 class SegImageProcessor:
     """One class for the three mappers: they differ in ground-truth handling only (not restated)."""
 

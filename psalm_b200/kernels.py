@@ -563,6 +563,68 @@ def rle_encode(masks):
 
 
 @_on_device
+def vos_pick(region_logits, stats):
+    """region_logits [K,Q] (model dtype), stats [Q,5] fp32 (postproc_fused's summed partials) -> (pick int32 [K],
+    score fp32 [K]): the per-object top-10 de-duplicating pick of eval_davis.py:443-453 (csrc/vos.cu)."""
+    _chk(region_logits, "vos_pick.region_logits")
+    _chk(stats, "vos_pick.stats")
+    K, Q = region_logits.shape
+    if stats.dtype != torch.float32 or tuple(stats.shape) != (Q, 5):
+        raise _lib.PsalmKernelError("vos_pick: stats must be fp32 [Q,5]")
+    pick = torch.empty(K, dtype=torch.int32, device=stats.device)
+    score = torch.empty(K, dtype=torch.float32, device=stats.device)
+    _lib.check(_lib.lib().psalm_vos_pick(_lib.ptr(region_logits), _lib.ptr(stats), _lib.ptr(pick), _lib.ptr(score), K, Q,
+                                         _lib.dtype_code(region_logits.dtype), _lib.stream_ptr(stats.device)),
+               "psalm_vos_pick")
+    _count()
+    return pick, score
+
+
+@_on_device
+def vos_fuse(masks, src_row, src_col, bits, row_prefix, count, fill=None, labels=None, area=None, inter=None):
+    """masks [K,H,W] fp32 (non-zero = set) at the output size.  Writes the padded-size bit masks bits [K,Hp,ceil(Wp/32)]
+    int32 (Pillow NEAREST through the index tables src_row [Hp] / src_col [Wp], -1 = zero), row_prefix [K,Hp+1] and
+    count [K]; with `labels` also the uint8 label map [H,W] (fill [K] int32), area [K] and inter [K,K] int32."""
+    for t, n in ((masks, "masks"), (src_row, "src_row"), (src_col, "src_col"), (bits, "bits"), (row_prefix, "row_prefix"),
+                 (count, "count")):
+        _chk(t, "vos_fuse." + n)
+    K, H, W = masks.shape
+    Hp, Wp = src_row.numel(), src_col.numel()
+    if masks.dtype != torch.float32 or tuple(bits.shape) != (K, Hp, (Wp + 31) // 32) or \
+            tuple(row_prefix.shape) != (K, Hp + 1) or count.numel() != K:
+        raise _lib.PsalmKernelError("vos_fuse: masks fp32 [K,H,W], bits [K,Hp,ceil(Wp/32)], row_prefix [K,Hp+1], count [K]")
+    if labels is not None:
+        for t, n in ((fill, "fill"), (labels, "labels"), (area, "area"), (inter, "inter")):
+            _chk(t, "vos_fuse." + n)
+        if labels.dtype != torch.uint8 or tuple(labels.shape) != (H, W) or fill.numel() != K or inter.numel() != K * K:
+            raise _lib.PsalmKernelError("vos_fuse: labels uint8 [H,W], fill [K], inter [K,K]")
+    p = lambda t: _lib.ptr(t) if t is not None else None  # noqa: E731
+    _lib.check(_lib.lib().psalm_vos_fuse(p(masks), p(fill), p(src_row), p(src_col), p(labels), p(area), p(inter), p(bits),
+                                         p(row_prefix), p(count), K, H, W, Hp, Wp, _lib.stream_ptr(masks.device)),
+               "psalm_vos_fuse")
+    _count(4 if labels is not None else 2)
+
+
+@_on_device
+def region_points_gather(bits, row_prefix, sel, mask_of_region, Hp, Wp):
+    """bits [M,Hp,ceil(Wp/32)] / row_prefix [M,Hp+1] (vos_fuse's layout), sel [R,P] int32 = index of the wanted set pixel
+    in nonzero() order, mask_of_region [R] int32 -> points [R,P,2] fp32 (y / Hp, x / Wp), bit-identical to
+    `m.nonzero() / torch.tensor([Hp, Wp])` of sample_region_points."""
+    for t, n in ((bits, "bits"), (row_prefix, "row_prefix"), (sel, "sel"), (mask_of_region, "mask_of_region")):
+        _chk(t, "region_points_gather." + n)
+    R, P = sel.shape
+    if sel.dtype != torch.int32 or mask_of_region.dtype != torch.int32 or mask_of_region.numel() != R or \
+            bits.shape[1:] != (Hp, (Wp + 31) // 32) or row_prefix.shape[1] != Hp + 1:
+        raise _lib.PsalmKernelError("region_points_gather: bad shapes / dtypes")
+    pts = torch.empty((R, P, 2), dtype=torch.float32, device=sel.device)
+    _lib.check(_lib.lib().psalm_region_points_gather(_lib.ptr(bits), _lib.ptr(row_prefix), _lib.ptr(sel),
+                                                     _lib.ptr(mask_of_region), _lib.ptr(pts), R, P, Hp, Wp,
+                                                     _lib.stream_ptr(sel.device)), "psalm_region_points_gather")
+    _count()
+    return pts
+
+
+@_on_device
 def rle_decode(chars, offsets, H, W):
     """rleFrString + rleDecode (csrc/rle.cu): strings chars[offsets[i]:offsets[i+1]] (uint8 / int64 CUDA tensors) ->
     uint8 [n,H,W] 0/1."""

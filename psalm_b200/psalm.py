@@ -914,11 +914,157 @@ class PSALM:
         return results
 
 
+class VideoFrame:
+    """Result of one `VideoSession.step`: what eval_davis.py:433-480 computes for the frame.
+    labels uint8 [H,W] on the device (`fused_pred_mask`, eval_davis.py:460), query_index int64 [K] and scores fp32 [K]
+    (the picked query and its score per object, :443-453), fill_numbers int64 [K], memory_updated (the IoU check of
+    :463-480 passed and the frame became the clip's memory; always False without memory)."""
+
+    def __init__(self, labels, query_index, scores, fill_numbers, memory_updated):
+        self.labels, self.query_index, self.scores = labels, query_index, scores
+        self.fill_numbers, self.memory_updated = fill_numbers, memory_updated
+
+
+class PendingFrame:
+    """Handle of a submitted `VideoSession.step_async`.  `result()` waits for the frame's one small device-to-host copy,
+    makes the memory decision and returns the `VideoFrame`.  Its `labels` stay valid until two more frames of the
+    session have been submitted."""
+
+    def __init__(self, sess, labels, host, done):
+        self.sess, self.labels, self.host, self.done = sess, labels, host, done
+        self._frame = None
+
+    def result(self):
+        if self._frame is None:
+            self._frame = self.sess._finish(self)
+        return self._frame
+
+
+def memory_check(area, inter):
+    """eval_davis.py:464-473 on the counts of the kept masks: False when any two objects i != j overlap with
+    IoU = |i & j| / |i | j| > 0.4.  An IoU of 0 / 0 (two empty masks) is NaN in numpy and fails no comparison."""
+    K = len(area)
+    for i in range(K):
+        for j in range(K):
+            if i != j:
+                union = int(area[i]) + int(area[j]) - int(inter[i][j])
+                if union > 0 and int(inter[i][j]) / union > 0.4:
+                    return False
+    return True
+
+
+class VideoSession:
+    """One clip opened by `PSALMForDAVISEval.open_video`: the DAVIS evaluation loop of eval_davis.py:388-480 with its
+    state on the device.  The first frame's projector tokens and region masks are kept for the whole clip; each
+    `step(images, seg_info)` encodes the frame once (Swin, projector, pixel decoder, decoder memory), pools the K regions
+    from the memory frame (the last frame whose prediction passed the IoU check) or from the first frame, runs the prompt
+    pass and the region heads, picks one query per object, fuses the label map and keeps the picked masks as the
+    candidate memory.  Valid until the next `open_video` / `open_image` on the same lane (a stale session raises
+    RuntimeError)."""
+
+    MAX_OBJECTS = 32
+
+    def __init__(self, model, lane, gen, bufs, first_counts, fills, with_memory):
+        self.model, self.lane, self.gen, self.bufs = model, lane, gen, bufs
+        self.K = len(fills)
+        self.first_counts, self.fills, self.with_memory = list(first_counts), fills, bool(with_memory)
+        self.mem_counts = None           # set pixels of the memory masks, None until a frame passes the check
+        self.pending = None              # the last submitted frame whose memory decision is not made yet
+        self.frames = 0
+        dev = model.device
+        oh, ow, H, W = bufs["geom"]
+        hv = bufs["hostvec_len"]
+        pin = dev.type == "cuda"
+        self._labels = [torch.empty((H, W), dtype=torch.uint8, device=dev) for _ in range(2)]
+        self._host = [torch.empty(hv, dtype=torch.int32, pin_memory=pin) for _ in range(2)]
+
+    def _check(self):
+        if self.model._lane_gen.get(self.lane) != self.gen:
+            raise RuntimeError("stale VideoSession: open_video / open_image was called again on lane %d" % self.lane)
+
+    @torch.no_grad()
+    def step(self, images, seg_info):
+        return self.step_async(images, seg_info).result()
+
+    @torch.no_grad()
+    def step_async(self, images, seg_info):
+        """Submit the next frame (images [1,3,H,W], float or uint8, as eval_seg; seg_info: the frame's mapper dict list).
+        The frame's image phase is enqueued first; then the previous frame's memory decision is made (its small copy
+        is waited for while the device encodes this frame), and the prompt phase follows."""
+        self._check()
+        m, b = self.model, self.bufs
+        if images.shape[0] != 1 or len(seg_info) != 1:
+            raise ValueError("step takes one frame (got %d)" % images.shape[0])
+        if tuple(images.shape[-2:]) != b["image_hw"]:
+            raise ValueError("frame size %s differs from the clip's %s" % (tuple(images.shape[-2:]), b["image_hw"]))
+        geom = m._geoms(b["image_hw"], seg_info, [PP.unpadded_box(seg_info[0]["padding_mask"])])[0]
+        if geom != b["geom"]:
+            raise ValueError("frame geometry %s differs from the clip's %s" % (geom, b["geom"]))
+        images_d = images.to(m.device, non_blocking=True)
+        if m.use_cuda_graph:
+            state = m._image_graphed(images_d, self.lane)
+        else:
+            with m._precision_scope():
+                state = m._image_core(images_d)
+        if self.pending is not None:
+            self.pending.result()
+        self._plan_inputs()
+        out = m._video_forward(state, b)
+        r = self.frames % 2
+        labels, host = self._labels[r], self._host[r]
+        labels.copy_(out["labels"])
+        host.copy_(out["hostvec"], non_blocking=True)
+        done = None
+        if m.device.type == "cuda":
+            done = torch.cuda.Event()
+            done.record(torch.cuda.current_stream(m.device))
+        self.pending = PendingFrame(self, labels, host, done)
+        self.frames += 1
+        return self.pending
+
+    def _plan_inputs(self):
+        """Host-planned inputs of the prompt phase: the 256 sample-point indices per region, drawn with the reference's
+        calls from the set-pixel counts of the source masks (memory or first frame), and the source slots."""
+        from .region import draw_point_indices
+        K, b = self.K, self.bufs
+        use_mem = self.with_memory and self.mem_counts is not None
+        sel = draw_point_indices(self.mem_counts if use_mem else self.first_counts)
+        slot = 1 if use_mem else 0
+        host = torch.cat([sel.view(-1), torch.arange(slot * K, slot * K + K, dtype=torch.int32),
+                          torch.full((K,), slot, dtype=torch.int32), torch.as_tensor(self.fills, dtype=torch.int32)])
+        b["inputs"].copy_(host, non_blocking=True)
+
+    def _finish(self, pending):
+        K, b = self.K, self.bufs
+        if pending.done is not None:
+            pending.done.synchronize()
+        hv = pending.host.numpy()
+        pick = hv[:K].astype("int64")
+        score = hv[K:2 * K].copy().view("float32")
+        area = hv[2 * K:3 * K]
+        inter = hv[3 * K:3 * K + K * K].reshape(K, K)
+        counts = hv[3 * K + K * K:4 * K + K * K].tolist()
+        updated = False
+        if self.with_memory and memory_check(area, inter):
+            # promote the candidate (this frame's tokens and kept masks) to the memory slot, in stream order: the next
+            # prompt phase, which overwrites the candidate, runs after these copies
+            b["src_tok"][1].copy_(b["src_tok"][2])
+            b["bits"][K:2 * K].copy_(b["bits"][2 * K:])
+            b["prefix"][K:2 * K].copy_(b["prefix"][2 * K:])
+            self.mem_counts = counts
+            updated = True
+        if self.pending is pending:
+            self.pending = None
+        return VideoFrame(pending.labels, torch.from_numpy(pick), torch.from_numpy(score),
+                          torch.as_tensor(self.fills, dtype=torch.int64), updated)
+
+
 class PSALMForDAVISEval(PSALM):
     """Video-object-segmentation variant (llava_phi.py:1477-2012, builder.py:47 'psalm_video'): the <region> prompts of
     the current frame are pooled from a VISUAL-PROMPT frame (`vp_images`, usually the first frame of the clip) with
     `seg_info[i]['instances'].vp_region_masks`; everything after the sequence splice is PSALM.eval_seg.  The reference's
-    `eval_seg` and `eval_video` of this class run the same computation."""
+    `eval_seg` and `eval_video` of this class run the same computation.  `open_video` runs the reference's whole
+    per-frame DAVIS loop (eval_davis.py:388-480) as a session."""
 
     def eval_seg(self, *args, vp_images=None, **kw):
         if vp_images is None:
@@ -926,3 +1072,136 @@ class PSALMForDAVISEval(PSALM):
         return super().eval_seg(*args, vp_images=vp_images, **kw)
 
     eval_video = eval_seg
+
+    @torch.no_grad()
+    def open_video(self, vp_images, seg_info, input_ids, attention_mask=None, lane=0, with_memory=True):
+        """Open a clip: vp_images [1,3,H,W] is the first (visual-prompt) frame, seg_info its mapper dict list with
+        `instances.vp_region_masks` [K,H,W] and `instances.vp_fill_number` [K], input_ids / attention_mask the DAVIS
+        prompt with K <region> tokens.  The frame is encoded once and its projector tokens kept for the clip.  Returns a
+        `VideoSession`; `with_memory` is eval_davis.py's flag.  K <= 32 and fill numbers in 1..255 (the label map is
+        uint8), else ValueError."""
+        if vp_images.shape[0] != 1 or len(seg_info) != 1:
+            raise ValueError("open_video takes one visual-prompt frame (got %d)" % vp_images.shape[0])
+        inst = seg_info[0]["instances"]
+        masks = inst.vp_region_masks
+        masks = (masks.tensor if hasattr(masks, "tensor") else masks).cpu()
+        fills = [int(f) for f in torch.as_tensor(inst.vp_fill_number).view(-1).tolist()]
+        K = len(fills)
+        if not 1 <= K <= VideoSession.MAX_OBJECTS or masks.shape[0] != K:
+            raise ValueError("open_video: %d objects with %d region masks (1..%d objects, one mask each)"
+                             % (K, masks.shape[0], VideoSession.MAX_OBJECTS))
+        if any(not 1 <= f <= 255 for f in fills):
+            raise ValueError("open_video: fill numbers must be in 1..255 (the label map is uint8), got %s" % fills)
+        image_hw = tuple(vp_images.shape[-2:])
+        if tuple(masks.shape[-2:]) != image_hw:
+            raise ValueError("open_video: region masks %s are not at the frame size %s" % (tuple(masks.shape[-2:]), image_hw))
+        if attention_mask is None:
+            attention_mask = torch.ones_like(input_ids, dtype=torch.bool)
+        plan = self._cached_plan(input_ids, attention_mask, image_hw, None, None, None, None, None)
+        if plan.B != 1 or plan.region_counts != (K,):
+            raise ValueError("open_video: the prompt needs one <region> token per object (%d objects, %s tokens)"
+                             % (K, plan.region_counts))
+        if "region_projector" not in self.proj:
+            raise KeyError("region prompts need region_projector.* in the checkpoint")
+        n_img = plan.n_img
+        if int(round(n_img ** 0.5)) ** 2 != n_img:
+            raise ValueError("region prompts need a square projector map (got %d tokens)" % n_img)
+        geom = self._geoms(image_hw, seg_info, [PP.unpadded_box(seg_info[0]["padding_mask"])])[0]
+        Hpad, Wpad = self._padded(image_hw)
+        if geom != (Hpad, Wpad, Hpad, Wpad):
+            from . import kernels
+            ps = self.cfg.swin.patch
+            H4, W4 = -(-image_hw[0] // ps), -(-image_hw[1] // ps)
+            if not kernels.postproc_crop_supported(self.num_queries, H4, W4, Hpad, Wpad, *geom, 0):
+                raise ValueError("open_video: geometry %s is outside the fused task-head kernel" % (geom,))
+        if not hasattr(self, "_lane_gen"):
+            self._lane_gen = {}
+        gen = self._lane_gen[lane] = self._lane_gen.get(lane, 0) + 1
+        key = (lane, image_hw, K, geom, _content_key(input_ids), _content_key(attention_mask))
+        bufs = self._lru("_video_bufs", key, lambda: self._video_buffers(plan, K, image_hw, geom), self.MAX_GRAPHS)
+        vp = vp_images.to(self.device, non_blocking=True)
+        if self.use_cuda_graph:
+            state = self._image_graphed(vp, lane)
+        else:
+            with self._precision_scope():
+                state = self._image_core(vp)
+        bufs["src_tok"][0].copy_(state["img_tok"][0])
+        self._first_frame_bits(bufs, masks, K)
+        return VideoSession(self, lane, gen, bufs, masks.flatten(1).sum(1).tolist(), fills, with_memory)
+
+    def _video_buffers(self, plan, K, image_hw, geom):
+        """Device buffers of a clip shape: token slots (0 first frame, 1 memory, 2 candidate), region mask bits in
+        three groups of K with the same roles, the host-planned inputs, the Pillow tables of the kept masks."""
+        from .image_processor import nearest_pad_tables
+        from .region import NUM_SAMPLE_POINT
+        dev = self.device
+        Hp, Wp = image_hw
+        oh, ow, H, W = geom
+        P = NUM_SAMPLE_POINT
+        rows, cols = nearest_pad_tables(H, W, (oh, ow), (Hp, Wp))
+        inputs = torch.zeros(K * P + 3 * K, dtype=torch.int32, device=dev)
+        return dict(plan=plan, K=K, image_hw=(Hp, Wp), geom=geom,
+                    src_tok=torch.zeros((3, plan.n_img, self.cfg.phi.hidden), dtype=self.dtype, device=dev),
+                    bits=torch.zeros((3 * K, Hp, (Wp + 31) // 32), dtype=torch.int32, device=dev),
+                    prefix=torch.zeros((3 * K, Hp + 1), dtype=torch.int32, device=dev),
+                    count=torch.zeros(3 * K, dtype=torch.int32, device=dev),
+                    inputs=inputs, sel=inputs[:K * P].view(K, P), mask_of_region=inputs[K * P:K * P + K],
+                    region_image=inputs[K * P + K:K * P + 2 * K], fill=inputs[K * P + 2 * K:],
+                    src_row=rows.to(dev), src_col=cols.to(dev), hostvec_len=4 * K + K * K)
+
+    def _first_frame_bits(self, bufs, masks, K):
+        """The first frame's region masks (already at the network input size) -> bit slot 0 (identity tables)."""
+        from . import kernels
+        Hp, Wp = bufs["image_hw"]
+        dev = self.device
+        kernels.vos_fuse(masks.to(dev, torch.float32).contiguous(), torch.arange(Hp, dtype=torch.int32, device=dev),
+                         torch.arange(Wp, dtype=torch.int32, device=dev), bufs["bits"][:K], bufs["prefix"][:K],
+                         bufs["count"][:K])
+
+    def _video_core(self, state, bufs):
+        """Prompt phase of one frame (capturable): region pooling from the session's token slots, the Phi prefill, the
+        heads, the decoder against the frame's memory, the region heads on the fused kernel (pass 1: per-query mask
+        scores; pass 2: the K picked masks), the pick, the label map and the candidate memory.  Returns the label map
+        and the one int32 vector the host reads: pick [K], score bits [K], area [K], inter [K*K], candidate counts [K]."""
+        from . import kernels
+        plan, K = bufs["plan"], bufs["K"]
+        Hp, Wp = bufs["image_hw"]
+        oh, ow, H, W = bufs["geom"]
+        Hpad, Wpad = self._padded((Hp, Wp))
+        with self._precision_scope():
+            img_tok = state["img_tok"]
+            side = int(round(img_tok.shape[1] ** 0.5))
+            bufs["src_tok"][2].copy_(img_tok[0])
+            pts = kernels.region_points_gather(bufs["bits"], bufs["prefix"], bufs["sel"], bufs["mask_of_region"], Hp, Wp)
+            feat = kernels.region_pool(bufs["src_tok"], pts, bufs["region_image"], side, side)
+            embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok, self.seg_query, feat)
+            hidden = self.model.phi(embeds, plan.attention_mask if plan.any_padding else None)
+            seg_q, SEG_emb, cls_emb = self._llm_heads(plan, hidden)
+            rows = F.linear(SEQ.gather_region_rows(plan, hidden), *self.proj["region_projector"])
+            out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
+                                                region_embedding_list=[rows], memory=state["mem"])
+            H4, W4 = state["mask_size"]
+            logits = out["pred_masks"][0].reshape(-1, H4, W4).contiguous()
+            crop = None if (oh, ow, H, W) == (Hpad, Wpad, Hpad, Wpad) else (Hpad, Wpad, oh, ow)
+            stats = kernels.postproc_fused(logits, H, W, crop=crop)["stats"]
+            pick, score = kernels.vos_pick(out["pred_region_logits"][0].contiguous(), stats)
+            masks = kernels.postproc_fused(logits, H, W, slot_query=pick, crop=crop)["inst_masks"]
+            labels = torch.empty((H, W), dtype=torch.uint8, device=logits.device)
+            area = torch.empty(K, dtype=torch.int32, device=logits.device)
+            inter = torch.empty((K, K), dtype=torch.int32, device=logits.device)
+            kernels.vos_fuse(masks, bufs["src_row"], bufs["src_col"], bufs["bits"][2 * K:], bufs["prefix"][2 * K:],
+                             bufs["count"][2 * K:], fill=bufs["fill"], labels=labels, area=area, inter=inter)
+            hostvec = torch.cat([pick, score.view(torch.int32), area, inter.view(-1), bufs["count"][2 * K:]])
+        return dict(labels=labels, hostvec=hostvec)
+
+    def _video_forward(self, state, bufs):
+        """The prompt phase, replayed from a CUDA graph per (clip buffers, image-graph state) with `use_cuda_graph`."""
+        if not self.use_cuda_graph:
+            return self._video_core(state, bufs)
+
+        def make():
+            g, out = self._capture(lambda: self._video_core(state, bufs))
+            return g, out, bufs, state
+        g, out, _, _ = self._lru("_video_graphs", (id(bufs), id(state)), make, self.MAX_GRAPHS)
+        g.replay()
+        return out

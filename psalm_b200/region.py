@@ -32,6 +32,26 @@ def sample_region_points(region_masks, num_sample_point=NUM_SAMPLE_POINT):
     return torch.stack(out).float()
 
 
+def draw_point_indices(counts, num_sample_point=NUM_SAMPLE_POINT):
+    """The random part of `sample_region_points` for masks with `counts` set pixels: [K, num_sample_point] int32 indices
+    into each mask's `nonzero()` rows, drawn with the same calls in the same order on the global CPU generator, so that
+    `m.nonzero()[idx] / wh` equals `sample_region_points` from the same generator state.  The masks themselves stay on the
+    device (kernels.region_points_gather turns the indices into points)."""
+    out = []
+    for n in counts:
+        n = int(n)
+        if n == 0:
+            raise ValueError("empty region mask (the reference prints 'error' and then fails in torch.randint)")
+        if n < num_sample_point:
+            idx = torch.cat((torch.arange(n), torch.randint(0, n, (num_sample_point - n,))))
+        elif n > num_sample_point:
+            idx = torch.randperm(n)[:num_sample_point]
+        else:
+            idx = torch.arange(n)
+        out.append(idx)
+    return torch.stack(out).to(torch.int32)
+
+
 def region_inputs(seg_info, region_points=None, attr="region_masks"):
     """seg_info: list of dicts with 'instances' (`.region_masks.tensor` [K,H,W], llava_phi.py:792; the DAVIS variant reads
     `.vp_region_masks`, :1664) -> (points [R,P,2] fp32, region_image [R] int32, counts).  `region_points`: optional
