@@ -199,7 +199,9 @@ __device__ __forceinline__ void xa_step(XaWarpState<T, NMT>& st, uint32_t sb, co
       const bool up0 = tmax0 > kRaise || (r0 == -INFINITY && tmax0 > -INFINITY);   // row-uniform over the quad
       const bool up1 = tmax1 > kRaise || (r1 == -INFINITY && tmax1 > -INFINITY);
       const float d0 = up0 ? tmax0 : 0.f, d1 = up1 ? tmax1 : 0.f;
-      const float c0 = xa_exp2(-d0), c1 = xa_exp2(-d1);
+      // -d > 0 only on a row's first open tile, where l and O are still 0: the clamp keeps 2^-d finite there (a tile
+      // maximum below -128 in the log2 domain would give inf, and 0 * inf = NaN in l and O); elsewhere -d <= 0
+      const float c0 = xa_exp2(fminf(-d0, 64.f)), c1 = xa_exp2(fminf(-d1, 64.f));
       if (up0) st.m_run[mt][0] = (r0 == -INFINITY ? 0.f : r0) + d0;
       if (up1) st.m_run[mt][1] = (r1 == -INFINITY ? 0.f : r1) + d1;
       st.l_run[mt][0] *= c0;
