@@ -24,8 +24,9 @@ class PagedKVCache:
         shape = (batch * self.max_pages, nh, page_size, hd)
         self.k = [torch.empty(shape, dtype=dtype, device=device) for _ in range(phi_cfg.layers)]
         self.v = [torch.empty(shape, dtype=dtype, device=device) for _ in range(phi_cfg.layers)]
-        bt = torch.arange(self.max_pages)[None, :] * batch + torch.arange(batch)[:, None]
-        self.block_table = bt.to(torch.int32).contiguous().to(device)
+        # built on the device (no host copy), so that a cache can also be allocated inside a CUDA graph capture
+        bt = torch.arange(self.max_pages * batch, dtype=torch.int32, device=device).view(self.max_pages, batch)
+        self.block_table = bt.t().contiguous()
         self.length = 0
         self.seq_lens = torch.zeros(batch, dtype=torch.int32, device=device)          # tokens already cached
         self.seq_lens_plus1 = torch.ones(batch, dtype=torch.int32, device=device)     # ... including the one being decoded

@@ -75,8 +75,8 @@ class PhiModel:
 
     def forward_suffix(self, inputs_embeds, prefix_cache, key_valid=None):
         """Prefill of B prompt suffixes behind one shared prefix whose K / V rows of every layer are in `prefix_cache` (a
-        generate.PagedKVCache of one sequence and one page, filled by `forward(..., cache=...)` and advanced by its length
-        P).  inputs_embeds [B,Ts,C] are positions P..P+Ts-1; key_valid [B,Ts] (True/1 = real token) or None ->
+        generate.PagedKVCache of one sequence and one page, filled by `forward(..., cache=...)`, whose `length` is the
+        prefix length P).  inputs_embeds [B,Ts,C] are positions P..P+Ts-1; key_valid [B,Ts] (True/1 = real token) or None ->
         last_hidden_state [B,Ts,C], the rows the unsplit prompts would give at those positions."""
         cfg, w = self.cfg, self.w
         B, T, C = inputs_embeds.shape

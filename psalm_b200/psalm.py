@@ -88,16 +88,14 @@ class ImageSession:
         self.image_hw, self.seg_info, self.boxes = image_hw, seg_info, boxes
         self.prefixes = OrderedDict()     # prefix input ids (bytes) -> PagedKVCache of its K / V
 
-    def _check(self):
-        if self.model._lane_gen.get(self.lane) != self.gen:
-            raise RuntimeError("stale ImageSession: open_image was called again on lane %d" % self.lane)
-
     def prefix_cache(self, split):
         """K / V of the shared prefix `split` (prefilled on first use, two most recent prefixes kept)."""
         key = split.prefix_ids.tobytes()
         cache = self.prefixes.get(key)
         if cache is None:
-            cache = self.model._prefix_for(self, split)
+            m = self.model
+            cache = m._phase("_prefix_graphs", (self.lane, key), lambda sp: m._prefix_core(self.state, sp),
+                             refresh=(split,), reads=(self.state,))
             while len(self.prefixes) >= self.MAX_PREFIXES:
                 self.prefixes.popitem(last=False)
             self.prefixes[key] = cache
@@ -115,8 +113,8 @@ class ImageSession:
     def eval_seg_async(self, prompts, is_thing_list=None, mask_format="dense"):
         if mask_format not in MASK_FORMATS:
             raise ValueError("mask_format must be one of %s, got %r" % (MASK_FORMATS, mask_format))
-        self._check()
         m = self.model
+        m._check_lane(self.lane, self.gen, "stale ImageSession: open_image was called again on lane %d")
         things = [p.get("is_thing_list", is_thing_list) for p in prompts]
         if m.panoptic_on and any(t is None for t in things):
             raise ValueError("is_thing_list need to be given")   # llava_phi.py:1337-1339
@@ -141,24 +139,15 @@ def _content_key(t):
     return (tuple(t.shape), str(t.dtype), t.numpy().tobytes())
 
 
-_PLAN_TENSORS = ("tok_ids", "img_pos", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool")
+# The device tensors a CUDA graph reads from a plan input of a phase (PSALM._phase), by plan type
+_GRAPH_TENSORS = {SEQ.SequencePlan: ("tok_ids", "img_pos", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool"),
+                  SEQ.PromptSplit: ("tok_ids", "img_pos")}
 
 
-def _graph_copy(plan, names=_PLAN_TENSORS):
-    """Shallow copy of a plan (SequencePlan / PromptSplit) with its own clones of the device tensors `names`, for a CUDA
-    graph to read: the cached plan they came from may be evicted and freed.  `_graph_refresh` fills them before a replay."""
-    static = copy.copy(plan)
-    for n in names:
-        t = getattr(plan, n)
-        setattr(static, n, None if t is None else t.clone())
-    return static
-
-
-def _graph_refresh(static, plan, names=_PLAN_TENSORS):
-    for n in names:
-        t = getattr(plan, n)
-        if t is not None:
-            getattr(static, n).copy_(t, non_blocking=True)
+def _plan_key(plan):
+    """The structure of a SequencePlan a captured graph is bound to (shapes and which optional rows exist)."""
+    return (plan.B, plan.T, plan.n_img, plan.any_padding, None if plan.cls_pool is None else tuple(plan.cls_pool.shape),
+            plan.refer_pool is not None, None if plan.pad_pos is None else int(plan.pad_pos.numel()))
 
 
 def attach_rle(results):
@@ -202,6 +191,7 @@ class PSALM:
                  seg_task="panoptic", use_cuda_graph=False):
         self._check_runtime(device)
         self.use_cuda_graph = use_cuda_graph
+        self._lane_gen = {}            # lane -> generation of its newest session (open_image / open_video)
         # one fused kernel for the task heads (16-bit storage); fp32 parity runs keep the exact torch path
         self._fused_postprocess = dtype != torch.float32
         self.overlap_branches = True   # pixel decoder || LLM prefill on two streams
@@ -335,11 +325,22 @@ class PSALM:
     def _region_features(self, img_tok, plan):
         """[R, hidden] pooled region features (region_pooling, context_cluster.py:333-400) from the projector tokens."""
         from . import kernels
-        n_img = img_tok.shape[1]
-        h = w = int(round(n_img ** 0.5))
-        if h * w != n_img:      # context_cluster.py:355 takes h = w = int(sqrt(n)): square maps only
+        side = self._region_side(img_tok.shape[1])
+        return kernels.region_pool(img_tok.contiguous(), plan.region_points, plan.region_image, side, side)
+
+    @staticmethod
+    def _region_side(n_img):
+        """Side of the projector map that region pooling reads: context_cluster.py:355 takes h = w = int(sqrt(n)), so
+        square maps only."""
+        side = int(round(n_img ** 0.5))
+        if side * side != n_img:
             raise ValueError("region prompts need a square projector map (got %d tokens)" % n_img)
-        return kernels.region_pool(img_tok.contiguous(), plan.region_points, plan.region_image, h, w)
+        return side
+
+    def _region_projector(self):
+        if "region_projector" not in self.proj:
+            raise KeyError("region prompts need region_projector.* in the checkpoint")
+        return self.proj["region_projector"]
 
     # ---- LlavaMetaForCausalLM surface --------------------------------------------------------------
     def get_model(self):
@@ -377,15 +378,17 @@ class PSALM:
         return toks, sizes, img_tok
 
     def _llm_heads(self, plan, hidden):
-        """(seg queries, SEG embedding, class-name embeddings) from the LLM's hidden states; None for a head the prompt
-        has no rows for."""
+        """(seg queries, SEG embedding, class-name embeddings, projected <region> rows) from the LLM's hidden states; None
+        for a head the prompt has no rows for."""
         seg_q = F.linear(SEQ.gather_seg_query(plan, hidden), *self.proj["seg_query_projector"])
-        SEG_emb = cls_emb = None
+        SEG_emb = cls_emb = region_rows = None
         if plan.refer_pool is not None:
             SEG_emb = F.linear(SEQ.pool(plan.refer_pool, hidden), *self.proj["SEG_token_projector"])
         if plan.cls_pool is not None:
             cls_emb = F.linear(SEQ.pool(plan.cls_pool, hidden), *self.proj["class_name_projector"])
-        return seg_q, SEG_emb, cls_emb
+        if plan.region_pos is not None:     # llava_phi.py:1385-1388: hidden states at the <region> rows -> region_projector
+            region_rows = F.linear(SEQ.gather_region_rows(plan, hidden), *self._region_projector())
+        return seg_q, SEG_emb, cls_emb, region_rows
 
     def _forward_core(self, images, plan, trace=None):
         toks, sizes, img_tok = self._swin_project(images)
@@ -413,13 +416,8 @@ class PSALM:
         # (cutting the batch into groups on separate streams so that the prefill GEMMs fill each other's tail waves was
         # measured and is slower: 20.8 ms / 21.9 ms per step of 4 for 2 / 4 groups against 19.5 ms)
         hidden = self.model.phi(embeds, plan.attention_mask if plan.any_padding else None)
-        seg_q, SEG_emb, cls_emb = self._llm_heads(plan, hidden)
-        region_emb = None
-        if plan.region_pos is not None:     # llava_phi.py:1385-1388: hidden states at the <region> rows -> region_projector
-            if "region_projector" not in self.proj:
-                raise KeyError("region prompts need region_projector.* in the checkpoint")
-            rows = F.linear(SEQ.gather_region_rows(plan, hidden), *self.proj["region_projector"])
-            region_emb = list(torch.split(rows, list(plan.region_counts), 0))
+        seg_q, SEG_emb, cls_emb, rows = self._llm_heads(plan, hidden)
+        region_emb = None if rows is None else list(torch.split(rows, list(plan.region_counts), 0))
         if branch is None:
             mask_features, ms, ms_sizes = self.pixel_decoder.forward_tokens(toks, sizes)
         else:   # join the pixel-decoder branch
@@ -468,6 +466,41 @@ class PSALM:
             out = fn()
         return g, out
 
+    def _phase(self, table, key, fn, refresh=(), reads=()):
+        """fn(*refresh), launched eagerly under `_precision_scope`, or with `use_cuda_graph` replayed from the CUDA graph of
+        `key` in the bounded LRU `self.<table>`; a graph's output is its static buffers, overwritten by its next replay.
+        `refresh`: the inputs that change per call (tensors, SequencePlans, PromptSplits); a graph reads its own copies of
+        their device tensors (`_GRAPH_TENSORS`), refreshed before every replay, since a cached input may be evicted and
+        freed while the graph lives.  `reads`: objects whose buffers fn reads as they are; their identities complete the
+        key and the entry holds them, so that an id cannot be handed to a new object while the graph lives."""
+        if not self.use_cuda_graph:
+            with self._precision_scope():
+                return fn(*refresh)
+
+        def tensors(x):
+            return [x] if isinstance(x, torch.Tensor) else [getattr(x, n) for n in _GRAPH_TENSORS[type(x)]]
+
+        def static_copy(x):
+            if isinstance(x, torch.Tensor):
+                return x.clone()
+            static = copy.copy(x)
+            for n in _GRAPH_TENSORS[type(x)]:
+                t = getattr(x, n)
+                setattr(static, n, None if t is None else t.clone())
+            return static
+
+        def make():
+            static = [static_copy(x) for x in refresh]
+            g, out = self._capture(lambda: fn(*static))
+            return g, static, out, reads
+        g, static, out, _ = self._lru(table, key + tuple(id(r) for r in reads), make, self.MAX_GRAPHS)
+        for s, x in zip(static, refresh):
+            for dst, src in zip(tensors(s), tensors(x)):
+                if src is not None:
+                    dst.copy_(src, non_blocking=True)
+        g.replay()
+        return out
+
     def _forward_post(self, images, plan, geoms):
         """forward_core, plus the device part of the fused task heads for the per-image geometries `geoms` when every
         image takes the fused kernel (capturable)."""
@@ -488,29 +521,30 @@ class PSALM:
         one by one from Python, plus ~150 extra tiny launches in its decoder).  `lane` selects an
         independent graph + static buffers so that several images can be in flight on different streams.
         `fuse_post` (`_fused_applies`): True (no crop / resize) or a tuple of per-image geometries puts the device part
-        of the fused task heads into the graph; False leaves the task heads to `post_process`."""
-        key = (lane, fuse_post, self.seg_task, float(self.object_mask_threshold), tuple(getattr(self, "is_thing_list", None) or ()), tuple(images.shape), str(images.dtype), plan.B,
-               plan.T, plan.n_img, plan.any_padding,
-               None if plan.cls_pool is None else tuple(plan.cls_pool.shape), plan.refer_pool is not None,
-               None if plan.pad_pos is None else int(plan.pad_pos.numel()))
+        of the fused task heads into the graph; False leaves the task heads to `post_process`.  Without `use_cuda_graph`
+        the same work is launched eagerly."""
+        key = (lane, fuse_post, self.seg_task, float(self.object_mask_threshold),
+               tuple(getattr(self, "is_thing_list", None) or ()), tuple(images.shape), str(images.dtype)) + _plan_key(plan)
         geoms = None
         if isinstance(fuse_post, tuple):
             geoms = fuse_post
         elif fuse_post:
             Hp, Wp = self._padded(images.shape[-2:])
             geoms = ((Hp, Wp, Hp, Wp),) * images.shape[0]      # no crop / resize
+        return self._phase("_graphs", key, lambda img, p: self._forward_post(img, p, geoms), refresh=(images, plan))
 
-        def make():
-            static_img, static_plan = images.clone(), _graph_copy(plan)
-            g, static_out = self._capture(lambda: self._forward_post(static_img, static_plan, geoms))
-            return g, static_img, static_plan, static_out
-        g, static_img, static_plan, static_out = self._lru("_graphs", key, make, self.MAX_GRAPHS)
-        static_img.copy_(images, non_blocking=True)
-        _graph_refresh(static_plan, plan)
-        g.replay()
-        return static_out
+    # ---- sessions: several prompts against one image, the frames of a clip ------------------------------------------
+    def _open_lane(self, lane):
+        """Generation of a new session on `lane`.  The phases of a lane share static buffers, so the new session ends the
+        lane's earlier ones."""
+        self._lane_gen[lane] = self._lane_gen.get(lane, 0) + 1
+        return self._lane_gen[lane]
 
-    # ---- several prompts against one image ------------------------------------------------------------------------
+    def _check_lane(self, lane, gen, stale):
+        """RuntimeError(`stale` % lane) when the session of generation `gen` on `lane` has been ended."""
+        if self._lane_gen.get(lane) != gen:
+            raise RuntimeError(stale % lane)
+
     @torch.no_grad()
     def open_image(self, images, seg_info, lane=0):
         """Encode ONE image (images [1,3,H,W]: float, uint8 or StagedImages, as eval_seg) for several prompts: Swin, the
@@ -518,25 +552,19 @@ class PSALM:
         `eval_seg(prompts)` runs only what depends on the prompts.  Opening an image ends the previous session of `lane`."""
         if images.shape[0] != 1 or len(seg_info) != 1:
             raise ValueError("open_image takes one image (got %d)" % images.shape[0])
-        staged = images if isinstance(images, StagedImages) else None
-        if staged is not None:
-            torch.cuda.current_stream(self.device).wait_event(staged.ready)
-            images_d = staged.tensor
-        else:
-            images_d = images.to(self.device, non_blocking=True)
-        if not hasattr(self, "_lane_gen"):
-            self._lane_gen = {}
-        gen = self._lane_gen[lane] = self._lane_gen.get(lane, 0) + 1
-        if self.use_cuda_graph:
-            state = self._image_graphed(images_d, lane)
-        else:
-            with self._precision_scope():
-                state = self._image_core(images_d)
-        if staged is not None:
-            staged.slot[1] = torch.cuda.Event()
-            staged.slot[1].record(torch.cuda.current_stream(self.device))
+        gen = self._open_lane(lane)
+        state = self._encode_image(self._device_images(images), lane)
+        self._release_staged(images)
         _, boxes = self._fused_applies(images.shape[-2:], seg_info)
         return ImageSession(self, lane, gen, state, tuple(images.shape[-2:]), list(seg_info), boxes)
+
+    # The session phases, graphed per lane: the image (per image shape and dtype), the prefix prefill (per image state and
+    # prefix content), the prompt pass (per image state, prefix cache, plan structure and task) and the video prompt
+    # phase (per image state and clip buffers).  Later phases read the static buffers of the earlier ones of the same
+    # lane, so a session is valid until the next open_image / open_video on its lane.
+    def _encode_image(self, images, lane):
+        return self._phase("_image_graphs", (lane, tuple(images.shape), str(images.dtype)), self._image_core,
+                           refresh=(images,))
 
     def _image_core(self, images):
         """Prompt-independent device work of one image (capturable)."""
@@ -546,34 +574,30 @@ class PSALM:
         return dict(swin=toks, swin_sizes=sizes, img_tok=img_tok, mask_features=mask_features, ms=ms, ms_sizes=ms_sizes,
                     mem=mem, mask_size=sizes[0])
 
-    def _prefix_core(self, state, split, cache=None):
-        """Prefill of the shared prefix (split.tok_ids / img_pos on the device): its K / V of every layer in a one-page
-        PagedKVCache whose page holds the P rows rounded up to 64 (head-major [nh, P_pad, hd] per layer, the layout
-        psalm_prefix_causal_attention reads).  Capturable when `cache` is given (allocated and advanced by the caller)."""
+    def _prefix_core(self, state, split):
+        """Prefill of the shared prefix (split.tok_ids / img_pos on the device) into a new PagedKVCache of one page that
+        holds the P rows rounded up to 64 (head-major [nh, P_pad, hd] per layer, the layout psalm_prefix_causal_attention
+        reads); capturable.  The rows are written from row 0 (the cache's seq_lens stay 0, so a replay writes the same
+        rows again); the host-side length P is what forward_suffix reads."""
         from .generate import PagedKVCache
-        fresh = cache is None
-        if fresh:
-            page = -(-split.P // 64) * 64
-            cache = PagedKVCache(self.cfg.phi, 1, page, self.dtype, self.device, page_size=page)
-        with self._precision_scope():
-            self.model.phi.forward(SEQ.prefix_embeds(split, self.model.embed_tokens, state["img_tok"]), None, cache=cache)
-        if fresh:
-            cache.advance(split.P)
+        page = -(-split.P // 64) * 64
+        cache = PagedKVCache(self.cfg.phi, 1, page, self.dtype, self.device, page_size=page)
+        self.model.phi.forward(SEQ.prefix_embeds(split, self.model.embed_tokens, state["img_tok"]), None, cache=cache)
+        cache.length = split.P
         return cache
 
     def _prompts_core(self, state, cache, plan):
         """Device work of K prompt suffixes (plan on device) against an opened image and its prefix cache (capturable).
         Returns forward_core's dict for the K prompts (pred_masks [K,Q,H4*W4], ...) and the suffix hidden states."""
-        with self._precision_scope():
-            img_tok = state["img_tok"]
-            embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok[:, :0], self.seg_query)
-            hidden = self.model.phi.forward_suffix(embeds, cache, plan.attention_mask if plan.any_padding else None)
-            seg_q, SEG_emb, cls_emb = self._llm_heads(plan, hidden)
-            out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
-                                                memory=state["mem"])
-            out["mask_size"] = state["mask_size"]
-            out["hidden"], out["seg_query"] = hidden, seg_q
-            return out
+        img_tok = state["img_tok"]
+        embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok[:, :0], self.seg_query)
+        hidden = self.model.phi.forward_suffix(embeds, cache, plan.attention_mask if plan.any_padding else None)
+        seg_q, SEG_emb, cls_emb, _ = self._llm_heads(plan, hidden)
+        out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
+                                            memory=state["mem"])
+        out["mask_size"] = state["mask_size"]
+        out["hidden"], out["seg_query"] = hidden, seg_q
+        return out
 
     def _cached_split(self, prompts, image_hw):
         """(host PromptSplit, device suffix plan) of a prompt set, cached by content like `_cached_plan`."""
@@ -597,65 +621,11 @@ class PSALM:
             h, w = (h + 1) // 2, (w + 1) // 2
         return ((h - 1) // 2 + 1) * ((w - 1) // 2 + 1)   # conv3x3 stride 2 pad 1 of the projector
 
-    # CUDA graphs of the session phases: the image (per lane, image shape and dtype), the prefix prefill (per lane, image
-    # key and prefix content) and the prompt pass (per lane, prefix, K, suffix length and plan structure, task heads).
-    # Later phases read the static buffers of the earlier ones of the same lane, so a session is valid until the next
-    # open_image on its lane.
-    def _image_graphed(self, images, lane):
-        key = (lane, tuple(images.shape), str(images.dtype))
-
-        def make():
-            static_img = images.clone()
-            g, state = self._capture(lambda: self._image_core(static_img))
-            return g, static_img, state
-        g, static_img, state = self._lru("_image_graphs", key, make, self.MAX_GRAPHS)
-        static_img.copy_(images, non_blocking=True)
-        g.replay()
-        return state
-
-    _PREFIX_TENSORS = ("tok_ids", "img_pos")
-
-    def _prefix_for(self, sess, split):
-        if not self.use_cuda_graph:
-            return self._prefix_core(sess.state, split)
-        # keyed by the image graph's state object: a re-captured image graph has new buffers; entries keep what they read
-        key = (sess.lane, id(sess.state), split.prefix_ids.tobytes())
-
-        def make():
-            from .generate import PagedKVCache
-            page = -(-split.P // 64) * 64
-            cache = PagedKVCache(self.cfg.phi, 1, page, self.dtype, self.device, page_size=page)
-            static = _graph_copy(split, self._PREFIX_TENSORS)
-            g, _ = self._capture(lambda: self._prefix_core(sess.state, static, cache))
-            # the replayed writes start at seq_lens (0): only the host-side length moves (forward_suffix reads it)
-            cache.length = split.P
-            return g, cache, sess.state, static
-        g, cache, _, static = self._lru("_prefix_graphs", key, make, self.MAX_GRAPHS)
-        _graph_refresh(static, split, self._PREFIX_TENSORS)
-        g.replay()
-        return cache
-
-    def _prompts_graphed(self, sess, cache, split, plan):
-        key = (sess.lane, id(sess.state), id(cache), plan.B, plan.T, plan.any_padding,
-               None if plan.cls_pool is None else tuple(plan.cls_pool.shape), plan.refer_pool is not None,
-               None if plan.pad_pos is None else int(plan.pad_pos.numel()), self.seg_task)
-
-        def make():
-            static_plan = _graph_copy(plan)
-            g, out = self._capture(lambda: self._prompts_core(sess.state, cache, static_plan))
-            return g, static_plan, out, (sess.state, cache)
-        g, static_plan, out, _ = self._lru("_prompt_graphs", key, make, self.MAX_GRAPHS)
-        _graph_refresh(static_plan, plan)
-        g.replay()
-        return out
-
     def _prompts_forward(self, sess, split, plan):
         """Run the prompt pass of a session and cut its output into one forward_core-style dict per prompt."""
         cache = sess.prefix_cache(split)
-        if self.use_cuda_graph:
-            out = self._prompts_graphed(sess, cache, split, plan)
-        else:
-            out = self._prompts_core(sess.state, cache, plan)
+        out = self._phase("_prompt_graphs", (sess.lane, self.seg_task) + _plan_key(plan),
+                          lambda p: self._prompts_core(sess.state, cache, p), refresh=(plan,), reads=(sess.state, cache))
         outs = []
         for k, ncls in enumerate(split.n_classes):
             cls = out["pred_class_name_logits"]
@@ -687,6 +657,22 @@ class PSALM:
             ready.record(st["stream"])
         return StagedImages(slot, ready)
 
+    def _device_images(self, images):
+        """`images` (a tensor or StagedImages) as a device tensor.  Float images are the reference contract (already
+        normalised by the mapper); uint8 images are raw pixel values, normalised on the device (coco_panoptic_mapper.py:161)
+        - 4x fewer bytes over PCIe.  A StagedImages upload is already in flight on the copy stream: the current stream
+        waits for it, and `_release_staged` must follow the pass that reads it."""
+        if isinstance(images, StagedImages):
+            torch.cuda.current_stream(self.device).wait_event(images.ready)
+            return images.tensor
+        return images.to(self.device, non_blocking=True)
+
+    def _release_staged(self, images):
+        """After the pass that reads `images` is enqueued: a staging buffer may be overwritten once that pass has run."""
+        if isinstance(images, StagedImages):
+            images.slot[1] = torch.cuda.Event()
+            images.slot[1].record(torch.cuda.current_stream(self.device))
+
     def make_plan(self, input_ids, attention_mask, image_hw, class_name_ids=None, cls_indices=None,
                   class_name_embedding_indices=None, token_refer_id=None, refer_embedding_indices=None):
         return SEQ.build_plan(input_ids, attention_mask, self.make_plan_n_img(image_hw), self.num_queries, class_name_ids, cls_indices,
@@ -712,9 +698,6 @@ class PSALM:
         """`mask_format`: "dense" (default) returns the reference's results; "rle" adds `instances.pred_masks_rle`, the
         COCO RLE dicts of `instances.pred_masks` encoded on the device (psalm_b200/rle.py), to every result with
         instances - what a COCO evaluator consumes, without copying the dense masks to the host."""
-        if self.panoptic_on:
-            assert is_thing_list is not None, "is_thing_list need to be given"   # llava_phi.py:1337-1339
-            self.is_thing_list = is_thing_list
         return self.eval_seg_async(region_points=region_points, vp_images=vp_images, input_ids=input_ids, attention_mask=attention_mask, images=images, seg_info=seg_info,
                                    class_name_ids=class_name_ids, class_name_embedding_indices=class_name_embedding_indices,
                                    cls_indices=cls_indices, token_refer_id=token_refer_id,
@@ -736,14 +719,7 @@ class PSALM:
         if self.panoptic_on:
             assert is_thing_list is not None, "is_thing_list need to be given"   # llava_phi.py:1337-1339
             self.is_thing_list = is_thing_list
-        staged = images if isinstance(images, StagedImages) else None
-        if staged is not None:   # upload already in flight on the copy stream (stage_images)
-            torch.cuda.current_stream(self.device).wait_event(staged.ready)
-            images_d = staged.tensor
-        else:
-            # float images are the reference contract (already normalised by the mapper); uint8 images are raw pixel
-            # values, normalised on the device (coco_panoptic_mapper.py:161) - 4x fewer bytes over PCIe
-            images_d = images.to(self.device, non_blocking=True)
+        images_d = self._device_images(images)
         plan = self._cached_plan(input_ids, attention_mask, images.shape[-2:], class_name_ids, cls_indices,
                                  class_name_embedding_indices, token_refer_id, refer_embedding_indices)
         has_regions = plan.region_pos is not None
@@ -760,10 +736,8 @@ class PSALM:
             out = self.forward_core_graphed(images_d, plan, lane=lane, fuse_post=fused)
         else:
             out = self.forward_core(images_d, plan)
+        self._release_staged(images)
         cur = torch.cuda.current_stream(self.device)
-        if staged is not None:   # the staging buffer may be overwritten once this pass has read it
-            staged.slot[1] = torch.cuda.Event()
-            staged.slot[1].record(cur)
         hostvecs = None
         if out.get("post") is not None:   # the integers of the host merge: device -> pinned memory, behind the pass
             if not hasattr(self, "_hostvec_pins"):
@@ -978,10 +952,6 @@ class VideoSession:
         self._labels = [torch.empty((H, W), dtype=torch.uint8, device=dev) for _ in range(2)]
         self._host = [torch.empty(hv, dtype=torch.int32, pin_memory=pin) for _ in range(2)]
 
-    def _check(self):
-        if self.model._lane_gen.get(self.lane) != self.gen:
-            raise RuntimeError("stale VideoSession: open_video / open_image was called again on lane %d" % self.lane)
-
     @torch.no_grad()
     def step(self, images, seg_info):
         return self.step_async(images, seg_info).result()
@@ -991,8 +961,8 @@ class VideoSession:
         """Submit the next frame (images [1,3,H,W], float or uint8, as eval_seg; seg_info: the frame's mapper dict list).
         The frame's image phase is enqueued first; then the previous frame's memory decision is made (its small copy
         is waited for while the device encodes this frame), and the prompt phase follows."""
-        self._check()
         m, b = self.model, self.bufs
+        m._check_lane(self.lane, self.gen, "stale VideoSession: open_video / open_image was called again on lane %d")
         if images.shape[0] != 1 or len(seg_info) != 1:
             raise ValueError("step takes one frame (got %d)" % images.shape[0])
         if tuple(images.shape[-2:]) != b["image_hw"]:
@@ -1000,16 +970,11 @@ class VideoSession:
         geom = m._geoms(b["image_hw"], seg_info, [PP.unpadded_box(seg_info[0]["padding_mask"])])[0]
         if geom != b["geom"]:
             raise ValueError("frame geometry %s differs from the clip's %s" % (geom, b["geom"]))
-        images_d = images.to(m.device, non_blocking=True)
-        if m.use_cuda_graph:
-            state = m._image_graphed(images_d, self.lane)
-        else:
-            with m._precision_scope():
-                state = m._image_core(images_d)
+        state = m._encode_image(images.to(m.device, non_blocking=True), self.lane)
         if self.pending is not None:
             self.pending.result()
         self._plan_inputs()
-        out = m._video_forward(state, b)
+        out = m._phase("_video_graphs", (), lambda: m._video_core(state, b), reads=(state, b))
         r = self.frames % 2
         labels, host = self._labels[r], self._host[r]
         labels.copy_(out["labels"])
@@ -1101,11 +1066,8 @@ class PSALMForDAVISEval(PSALM):
         if plan.B != 1 or plan.region_counts != (K,):
             raise ValueError("open_video: the prompt needs one <region> token per object (%d objects, %s tokens)"
                              % (K, plan.region_counts))
-        if "region_projector" not in self.proj:
-            raise KeyError("region prompts need region_projector.* in the checkpoint")
-        n_img = plan.n_img
-        if int(round(n_img ** 0.5)) ** 2 != n_img:
-            raise ValueError("region prompts need a square projector map (got %d tokens)" % n_img)
+        self._region_projector()
+        self._region_side(plan.n_img)
         geom = self._geoms(image_hw, seg_info, [PP.unpadded_box(seg_info[0]["padding_mask"])])[0]
         Hpad, Wpad = self._padded(image_hw)
         if geom != (Hpad, Wpad, Hpad, Wpad):
@@ -1114,17 +1076,10 @@ class PSALMForDAVISEval(PSALM):
             H4, W4 = -(-image_hw[0] // ps), -(-image_hw[1] // ps)
             if not kernels.postproc_crop_supported(self.num_queries, H4, W4, Hpad, Wpad, *geom, 0):
                 raise ValueError("open_video: geometry %s is outside the fused task-head kernel" % (geom,))
-        if not hasattr(self, "_lane_gen"):
-            self._lane_gen = {}
-        gen = self._lane_gen[lane] = self._lane_gen.get(lane, 0) + 1
+        gen = self._open_lane(lane)
         key = (lane, image_hw, K, geom, _content_key(input_ids), _content_key(attention_mask))
         bufs = self._lru("_video_bufs", key, lambda: self._video_buffers(plan, K, image_hw, geom), self.MAX_GRAPHS)
-        vp = vp_images.to(self.device, non_blocking=True)
-        if self.use_cuda_graph:
-            state = self._image_graphed(vp, lane)
-        else:
-            with self._precision_scope():
-                state = self._image_core(vp)
+        state = self._encode_image(vp_images.to(self.device, non_blocking=True), lane)
         bufs["src_tok"][0].copy_(state["img_tok"][0])
         self._first_frame_bits(bufs, masks, K)
         return VideoSession(self, lane, gen, bufs, masks.flatten(1).sum(1).tolist(), fills, with_memory)
@@ -1168,40 +1123,26 @@ class PSALMForDAVISEval(PSALM):
         Hp, Wp = bufs["image_hw"]
         oh, ow, H, W = bufs["geom"]
         Hpad, Wpad = self._padded((Hp, Wp))
-        with self._precision_scope():
-            img_tok = state["img_tok"]
-            side = int(round(img_tok.shape[1] ** 0.5))
-            bufs["src_tok"][2].copy_(img_tok[0])
-            pts = kernels.region_points_gather(bufs["bits"], bufs["prefix"], bufs["sel"], bufs["mask_of_region"], Hp, Wp)
-            feat = kernels.region_pool(bufs["src_tok"], pts, bufs["region_image"], side, side)
-            embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok, self.seg_query, feat)
-            hidden = self.model.phi(embeds, plan.attention_mask if plan.any_padding else None)
-            seg_q, SEG_emb, cls_emb = self._llm_heads(plan, hidden)
-            rows = F.linear(SEQ.gather_region_rows(plan, hidden), *self.proj["region_projector"])
-            out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
-                                                region_embedding_list=[rows], memory=state["mem"])
-            H4, W4 = state["mask_size"]
-            logits = out["pred_masks"][0].reshape(-1, H4, W4).contiguous()
-            crop = None if (oh, ow, H, W) == (Hpad, Wpad, Hpad, Wpad) else (Hpad, Wpad, oh, ow)
-            stats = kernels.postproc_fused(logits, H, W, crop=crop)["stats"]
-            pick, score = kernels.vos_pick(out["pred_region_logits"][0].contiguous(), stats)
-            masks = kernels.postproc_fused(logits, H, W, slot_query=pick, crop=crop)["inst_masks"]
-            labels = torch.empty((H, W), dtype=torch.uint8, device=logits.device)
-            area = torch.empty(K, dtype=torch.int32, device=logits.device)
-            inter = torch.empty((K, K), dtype=torch.int32, device=logits.device)
-            kernels.vos_fuse(masks, bufs["src_row"], bufs["src_col"], bufs["bits"][2 * K:], bufs["prefix"][2 * K:],
-                             bufs["count"][2 * K:], fill=bufs["fill"], labels=labels, area=area, inter=inter)
-            hostvec = torch.cat([pick, score.view(torch.int32), area, inter.view(-1), bufs["count"][2 * K:]])
+        img_tok = state["img_tok"]
+        side = self._region_side(img_tok.shape[1])
+        bufs["src_tok"][2].copy_(img_tok[0])
+        pts = kernels.region_points_gather(bufs["bits"], bufs["prefix"], bufs["sel"], bufs["mask_of_region"], Hp, Wp)
+        feat = kernels.region_pool(bufs["src_tok"], pts, bufs["region_image"], side, side)
+        embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok, self.seg_query, feat)
+        hidden = self.model.phi(embeds, plan.attention_mask if plan.any_padding else None)
+        seg_q, SEG_emb, cls_emb, rows = self._llm_heads(plan, hidden)
+        out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
+                                            region_embedding_list=[rows], memory=state["mem"])
+        H4, W4 = state["mask_size"]
+        logits = out["pred_masks"][0].reshape(-1, H4, W4).contiguous()
+        crop = None if (oh, ow, H, W) == (Hpad, Wpad, Hpad, Wpad) else (Hpad, Wpad, oh, ow)
+        stats = kernels.postproc_fused(logits, H, W, crop=crop)["stats"]
+        pick, score = kernels.vos_pick(out["pred_region_logits"][0].contiguous(), stats)
+        masks = kernels.postproc_fused(logits, H, W, slot_query=pick, crop=crop)["inst_masks"]
+        labels = torch.empty((H, W), dtype=torch.uint8, device=logits.device)
+        area = torch.empty(K, dtype=torch.int32, device=logits.device)
+        inter = torch.empty((K, K), dtype=torch.int32, device=logits.device)
+        kernels.vos_fuse(masks, bufs["src_row"], bufs["src_col"], bufs["bits"][2 * K:], bufs["prefix"][2 * K:],
+                         bufs["count"][2 * K:], fill=bufs["fill"], labels=labels, area=area, inter=inter)
+        hostvec = torch.cat([pick, score.view(torch.int32), area, inter.view(-1), bufs["count"][2 * K:]])
         return dict(labels=labels, hostvec=hostvec)
-
-    def _video_forward(self, state, bufs):
-        """The prompt phase, replayed from a CUDA graph per (clip buffers, image-graph state) with `use_cuda_graph`."""
-        if not self.use_cuda_graph:
-            return self._video_core(state, bufs)
-
-        def make():
-            g, out = self._capture(lambda: self._video_core(state, bufs))
-            return g, out, bufs, state
-        g, out, _, _ = self._lru("_video_graphs", (id(bufs), id(state)), make, self.MAX_GRAPHS)
-        g.replay()
-        return out

@@ -151,6 +151,36 @@ def test_cuda_graphs_of_different_sizes_and_batches_alternate():
     assert 3 <= len(graphed._graphs) <= 6        # one graph per (size, batch, prompt length) key; none evicted
 
 
+def test_cuda_graph_replays_a_prompt_whose_plan_left_the_plan_cache():
+    """More referring prompts of one structure than the plan cache holds (MAX_PLANS): one forward graph serves them all,
+    and replaying it for the first prompt after that prompt's cached plan was evicted and freed still gives the eager
+    results - the graph reads its own copies of the plan tensors, refreshed from the live plan before each replay."""
+    from psalm_b200.psalm import PSALM
+    sd = synth.synth_state_dict(SMALL, seed=5)
+    eager = PSALM(sd, SMALL, torch.bfloat16, "cuda", "referring", use_cuda_graph=False)
+    graphed = PSALM(sd, SMALL, torch.bfloat16, "cuda", "referring", use_cuda_graph=True)
+    inp = synth.synth_inputs(batch=1, height=192, width=192, task="referring", refer_len=9, seed=6)
+    g = torch.Generator().manual_seed(0)
+    refers = []
+    for _ in range(graphed.MAX_PLANS + 2):     # same length, different refer tokens: one graph key, distinct plans
+        r = inp["token_refer_id"][0].clone()
+        r[:-1] = torch.randint(5, 50000, (r.numel() - 1,), generator=g)
+        refers.append(r)
+
+    def run(m, refer):
+        res = m.eval_seg(input_ids=inp["input_ids"], attention_mask=inp["attention_mask"], images=inp["images"],
+                         seg_info=inp["seg_info"], token_refer_id=[refer],
+                         refer_embedding_indices=inp["refer_embedding_indices"])
+        torch.cuda.synchronize()
+        return res[0]["instances"].scores.clone(), res[0]["instances"].pred_masks.clone()
+    for r in refers:
+        run(graphed, r)
+    assert len(graphed._graphs) == 1 and len(graphed._plans) == graphed.MAX_PLANS
+    for r in (refers[0], refers[-1]):
+        (a, am), (b, bm) = run(graphed, r), run(eager, r)
+        assert torch.allclose(a, b, rtol=1e-5, atol=1e-7) and torch.equal(am, bm)
+
+
 def _oracle(sd, inp, task):
     from oracle import psalm_oracle as O
     phi = dict(hidden=256, layers=2, heads=4, inter=1024, eps=1e-5, theta=10000.0, rotary_frac=0.5)
