@@ -363,7 +363,19 @@ int psalm_rle_decode(const uint8_t* chars, const int64_t* byte_off, uint32_t* en
  * psalm_region_points_gather (region.py sample_region_points = context_cluster.py:31-40, :349-352): for region r and
  *   point p, the sel[r,p]-th set pixel (row-major, the order of nonzero()) of mask mask_of_region[r] of bits /
  *   row_prefix (layout of psalm_vos_fuse, M masks) -> points [R,P,2] fp32 = (y / Hp, x / Wp), IEEE divisions.  The
- *   caller draws sel on the host with the reference's randint / randperm calls. */
+ *   caller draws sel on the host with the reference's randint / randperm calls.
+ * psalm_visual_prompt_raster (the region-mask path of coco_instance_mapper.py:233-251: enhance_with_circles :17-33, then
+ *   transforms.apply_segmentation = Pillow NEAREST + FixedSizeCrop zero padding): src [K,H0,W0] uint8 = the prompt
+ *   masks at the original size (boxes painted half-open as datasets/bulid_COCO_Interactivate.py:72 does), radius [K]
+ *   int32 (10 point, 5 scribble, 0 box / mask), src_row [Hp] / src_col [Wp] the NEAREST + padding tables of
+ *   psalm_vos_fuse.  With r > 0 the pixels equal to 1 seed a disk dx^2 + dy^2 <= r^2 (draw_circle's sqrt(.) <= r),
+ *   clipped at the image border; with r = 0 the non-zero pixels are resized as they are.  Writes bits / row_prefix /
+ *   count in the layout of psalm_vos_fuse (what psalm_region_points_gather reads); src_bits [K,H0,ceil(W0/32)] uint32
+ *   is workspace.  The dilated mask is never built: output pixel (y, x) is set when a seed lies within r of
+ *   (src_row[y], src_col[x]). */
+int psalm_visual_prompt_raster(const uint8_t* src, const int* radius, const int* src_row, const int* src_col,
+                               uint32_t* src_bits, uint32_t* bits, int* row_prefix, int* count, int K, int H0, int W0,
+                               int Hp, int Wp, void* stream);
 int psalm_vos_pick(const void* region_logits, const float* stats, int* pick, float* score, int K, int Q, int dtype,
                    void* stream);
 int psalm_vos_fuse(const float* masks, const int* fill, const int* src_row, const int* src_col, uint8_t* labels,

@@ -78,6 +78,7 @@ SIGNATURES = {
     "psalm_vos_pick": ([_c_vp] * 4 + [_c_i] * 3 + [_c_vp], _c_i),
     "psalm_vos_fuse": ([_c_vp] * 10 + [_c_i] * 5 + [_c_vp], _c_i),
     "psalm_region_points_gather": ([_c_vp] * 5 + [_c_i] * 4 + [_c_vp], _c_i),
+    "psalm_visual_prompt_raster": ([_c_vp] * 8 + [_c_i] * 5 + [_c_vp], _c_i),
 }
 
 

@@ -7,6 +7,9 @@
 //                        memory check (:463-473), one bit per object per pixel;
 //   vos_bits_kernel      detectron2's ResizeTransform.apply_segmentation (Pillow NEAREST) + FixedSizeCrop zero padding of
 //   + vos_prefix_kernel  the kept masks (:406-408) as a bit mask at the network input size, with per-row set counts;
+//   vp_pack_kernel       visual prompts (click, scribble, box, mask) at the original image size: enhance_with_circles
+//   + vp_raster_kernel   (coco_instance_mapper.py:17-33) + the mapper's NEAREST resize and padding (:250), straight
+//                        into the bit layout of vos_bits_kernel (the dilated mask is never built);
 //   region_points_gather_kernel  "the i-th set pixel in nonzero() order" -> (y / H, x / W) for the host-drawn indices of
 //                        sample_region_points (psalm_b200/region.py = context_cluster.py:31-40, :349-352).
 #include "common.cuh"
@@ -169,6 +172,76 @@ __global__ void __launch_bounds__(32) vos_prefix_kernel(int* __restrict__ row_pr
   if (lane == 31) count[k] = incl;
 }
 
+// Visual prompts (coco_instance_mapper.py:17-33, :233-251): enhance_with_circles (a disk of radius r around every
+// source pixel equal to 1), then Pillow NEAREST + zero padding.  NEAREST reads one source pixel per output pixel, so the
+// dilated mask is never built: output pixel (y, x) is set when a seed lies in the disk around (src_row[y], src_col[x]).
+// draw_circle's float64 test sqrt(dx^2 + dy^2) <= r equals the integer test dx^2 + dy^2 <= r^2 for an integer r
+// (sqrt is correctly rounded and r^2 is exact), so row dy of the disk is the span |dx| <= isqrt(r^2 - dy^2).
+
+// One warp per (source row, region): the seeds as bits (== 1 for a dilated region, != 0 for r = 0, where the mask is
+// resized as it is).
+__global__ void __launch_bounds__(256) vp_pack_kernel(const uint8_t* __restrict__ src, const int* __restrict__ radius,
+                                                      uint32_t* __restrict__ src_bits, int H0, int W0) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int y = blockIdx.x * (blockDim.x >> 5) + warp, k = blockIdx.y;
+  if (y >= H0) return;
+  const int S32 = (W0 + 31) >> 5;
+  const bool ones_only = radius[k] > 0;
+  const uint8_t* row = src + ((size_t)k * H0 + y) * W0;
+  uint32_t* out = src_bits + ((size_t)k * H0 + y) * S32;
+  for (int w = 0; w < S32; ++w) {
+    const int x = (w << 5) + lane;
+    const uint8_t v = x < W0 ? row[x] : 0;
+    const unsigned b = __ballot_sync(0xffffffffu, ones_only ? v == 1 : v != 0);
+    if (lane == 0) out[w] = b;
+  }
+}
+
+__device__ __forceinline__ int isqrt_floor(int v) {
+  int h = (int)sqrtf((float)v);
+  while (h * h > v) --h;
+  while ((h + 1) * (h + 1) <= v) ++h;
+  return h;
+}
+
+// One warp per (padded row, region), lane i of a 32-pixel step tests output column 32 w + i: for every disk row dy the
+// span [sx - h, sx + h] (clipped at the border) is tested word by word against the seed bits; the ballot is the output
+// word.  Lane 0 keeps the row's set count for vos_prefix_kernel.
+__global__ void __launch_bounds__(256) vp_raster_kernel(const uint32_t* __restrict__ src_bits, const int* __restrict__ radius,
+                                                        const int* __restrict__ src_row, const int* __restrict__ src_col,
+                                                        uint32_t* __restrict__ bits, int* __restrict__ row_prefix, int H0,
+                                                        int W0, int Hp, int Wp) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int y = blockIdx.x * (blockDim.x >> 5) + warp, k = blockIdx.y;
+  if (y >= Hp) return;
+  const int W32 = (Wp + 31) >> 5, S32 = (W0 + 31) >> 5;
+  const int r = radius[k], sy = src_row[y];
+  const uint32_t* seeds = src_bits + (size_t)k * H0 * S32;
+  uint32_t* out = bits + ((size_t)k * Hp + y) * W32;
+  int n = 0;
+  for (int w = 0; w < W32; ++w) {
+    const int x = (w << 5) + lane;
+    const int sx = x < Wp ? src_col[x] : -1;
+    bool on = false;
+    if (sy >= 0 && sx >= 0) {
+      const int dy1 = min(r, H0 - 1 - sy);
+      for (int dy = max(-r, -sy); dy <= dy1 && !on; ++dy) {
+        const int h = isqrt_floor(r * r - dy * dy);
+        const int lo = max(sx - h, 0), hi = min(sx + h, W0 - 1);
+        const uint32_t* row = seeds + (size_t)(sy + dy) * S32;
+        for (int wi = lo >> 5; wi <= (hi >> 5) && !on; ++wi) {
+          const int b0 = max(lo - (wi << 5), 0), b1 = min(hi - (wi << 5), 31);
+          on = (row[wi] & (0xffffffffu >> (31 - b1)) & (0xffffffffu << b0)) != 0u;
+        }
+      }
+    }
+    const unsigned v = __ballot_sync(0xffffffffu, on);
+    if (lane == 0) out[w] = v;
+    n += __popc(v);
+  }
+  if (lane == 0) row_prefix[(size_t)k * (Hp + 1) + y + 1] = n;
+}
+
 // One thread per (region, point): binary search of the row holding the sel-th set pixel, then the words of that row.
 __global__ void __launch_bounds__(256) region_points_gather_kernel(const uint32_t* __restrict__ bits,
                                                                    const int* __restrict__ row_prefix,
@@ -256,6 +329,22 @@ extern "C" int psalm_vos_fuse(const float* masks, const int* fill, const int* sr
   }
   vos_bits_kernel<<<dim3((Hp + 7) / 8, K), 256, 0, st>>>(masks, src_row, src_col, bits, row_prefix, H, W, Hp, Wp);
   if (int rc = check_launch("vos_bits_kernel")) return rc;
+  vos_prefix_kernel<<<K, 32, 0, st>>>(row_prefix, count, Hp);
+  return check_launch("vos_prefix_kernel");
+}
+
+extern "C" int psalm_visual_prompt_raster(const uint8_t* src, const int* radius, const int* src_row, const int* src_col,
+                                          uint32_t* src_bits, uint32_t* bits, int* row_prefix, int* count, int K, int H0,
+                                          int W0, int Hp, int Wp, void* stream) {
+  PSALM_REQUIRE(src && radius && src_row && src_col && src_bits && bits && row_prefix && count,
+                "visual_prompt_raster: null pointer");
+  PSALM_REQUIRE(K > 0 && H0 > 0 && W0 > 0 && Hp > 0 && Wp > 0, "visual_prompt_raster: bad shape");
+  cudaStream_t st = (cudaStream_t)stream;
+  vp_pack_kernel<<<dim3((H0 + 7) / 8, K), 256, 0, st>>>(src, radius, src_bits, H0, W0);
+  if (int rc = check_launch("vp_pack_kernel")) return rc;
+  vp_raster_kernel<<<dim3((Hp + 7) / 8, K), 256, 0, st>>>(src_bits, radius, src_row, src_col, bits, row_prefix, H0, W0,
+                                                          Hp, Wp);
+  if (int rc = check_launch("vp_raster_kernel")) return rc;
   vos_prefix_kernel<<<K, 32, 0, st>>>(row_prefix, count, Hp);
   return check_launch("vos_prefix_kernel");
 }

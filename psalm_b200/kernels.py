@@ -625,6 +625,31 @@ def region_points_gather(bits, row_prefix, sel, mask_of_region, Hp, Wp):
 
 
 @_on_device
+def visual_prompt_raster(src, radius, src_row, src_col):
+    """src uint8 [K,H0,W0] prompt masks at the original size, radius int32 [K] (0 = no dilation), src_row [Hp] / src_col
+    [Wp] int32 NEAREST + padding tables -> (bits int32 [K,Hp,ceil(Wp/32)], row_prefix int32 [K,Hp+1], count int32 [K]):
+    enhance_with_circles, resize and pad of the reference mapper, in vos_fuse's layout (csrc/vos.cu)."""
+    for t, n in ((src, "src"), (radius, "radius"), (src_row, "src_row"), (src_col, "src_col")):
+        _chk(t, "visual_prompt_raster." + n)
+    K, H0, W0 = src.shape
+    Hp, Wp = src_row.numel(), src_col.numel()
+    if src.dtype != torch.uint8 or radius.dtype != torch.int32 or radius.numel() != K or \
+            src_row.dtype != torch.int32 or src_col.dtype != torch.int32:
+        raise _lib.PsalmKernelError("visual_prompt_raster: src uint8 [K,H0,W0], radius int32 [K], int32 tables")
+    dev = src.device
+    src_bits = torch.empty((K, H0, (W0 + 31) // 32), dtype=torch.int32, device=dev)
+    bits = torch.empty((K, Hp, (Wp + 31) // 32), dtype=torch.int32, device=dev)
+    row_prefix = torch.empty((K, Hp + 1), dtype=torch.int32, device=dev)
+    count = torch.empty(K, dtype=torch.int32, device=dev)
+    p = _lib.ptr
+    _lib.check(_lib.lib().psalm_visual_prompt_raster(p(src), p(radius), p(src_row), p(src_col), p(src_bits), p(bits),
+                                                     p(row_prefix), p(count), K, H0, W0, Hp, Wp, _lib.stream_ptr(dev)),
+               "psalm_visual_prompt_raster")
+    _count(3)
+    return bits, row_prefix, count
+
+
+@_on_device
 def rle_decode(chars, offsets, H, W):
     """rleFrString + rleDecode (csrc/rle.cu): strings chars[offsets[i]:offsets[i+1]] (uint8 / int64 CUDA tensors) ->
     uint8 [n,H,W] 0/1."""

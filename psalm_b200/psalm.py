@@ -63,7 +63,8 @@ class PendingSeg:
 
     def result(self):
         m = self.model
-        torch.cuda.current_stream(m.device).wait_event(self.done)
+        if self.done is not None:
+            torch.cuda.current_stream(m.device).wait_event(self.done)
         if any(hostvecs is not None for _, hostvecs, _ in self.parts):
             self.done.synchronize()                          # pinned host vectors are complete
         results = None
@@ -88,6 +89,20 @@ class ImageSession:
         self.image_hw, self.seg_info, self.boxes = image_hw, seg_info, boxes
         self.prefixes = OrderedDict()     # prefix input ids (bytes) -> PagedKVCache of its K / V
 
+    def _region_inputs(self, regions):
+        """The regions of all prompts of a call, rasterised in one batch at the session's geometry (original size, un-padded
+        box, input size) -> (bits, row_prefix, sample-point indices [R,256] on the device).  The set-pixel counts come to
+        the host (the reference draws its points there), and the indices are drawn region by region in prompt order: the
+        draws of per-prompt eval_seg calls made in that order from the same generator."""
+        from .region import draw_point_indices, rasterize_visual_prompts
+        m = self.model
+        info = self.seg_info[0]
+        H, W = self.image_hw
+        bits, prefix, count = rasterize_visual_prompts(regions, info.get("height", H), info.get("width", W),
+                                                       tuple(self.boxes[0]), (H, W), m.device)
+        sel = draw_point_indices(count.tolist())
+        return bits, prefix, sel.to(m.device)
+
     def prefix_cache(self, split):
         """K / V of the shared prefix `split` (prefilled on first use, two most recent prefixes kept)."""
         key = split.prefix_ids.tobytes()
@@ -106,7 +121,15 @@ class ImageSession:
     def eval_seg(self, prompts, is_thing_list=None, mask_format="dense"):
         """results[k] == model.eval_seg(images, seg_info, **prompts[k])[0] (same structure; values within the tolerances
         of a split prefill).  A prompt dict may carry its own `is_thing_list` (panoptic prompts with different class
-        lists); it overrides the call-level one."""
+        lists); it overrides the call-level one.
+
+        Interactive segmentation (the "region" task): a prompt with K <region> tokens carries `visual_prompts`, K
+        (kind, source) pairs at the original image size - kind "point", "scribble", "box" or "mask"; source a COCO RLE
+        dict, a binary [height, width] tensor, a (row, col) click or a (min_row, min_col, max_row, max_col) box
+        (region.rasterize_visual_prompts).  The regions are rasterised on the device as the reference mapper prepares
+        them (coco_instance_mapper.py:233-251) and their sample points are drawn like eval_seg's, prompt by prompt, from
+        the global CPU generator; the result is eval_seg's for the region task (instances with pred_masks [Q,H,W] and
+        scores [Q,K]; `gt` when the opened image's seg_info carries instances.gt_masks)."""
         return self.eval_seg_async(prompts, is_thing_list, mask_format).result()
 
     @torch.no_grad()
@@ -118,10 +141,24 @@ class ImageSession:
         things = [p.get("is_thing_list", is_thing_list) for p in prompts]
         if m.panoptic_on and any(t is None for t in things):
             raise ValueError("is_thing_list need to be given")   # llava_phi.py:1337-1339
+        visual = any("visual_prompts" in p for p in prompts)
+        if visual and not m.region_on:
+            raise ValueError("visual_prompts need the model in the \"region\" task (got %r)" % m.seg_task)
         split, plan = m._cached_split(prompts, self.image_hw)
-        outs = m._prompts_forward(self, split, plan)
-        done = torch.cuda.Event()
-        done.record(torch.cuda.current_stream(m.device))
+        region = None
+        if visual and plan.region_counts is not None:
+            vps = [p.get("visual_prompts", ()) for p in prompts]
+            if tuple(len(v) for v in vps) != plan.region_counts:
+                raise ValueError("visual_prompts: %s regions for %s <region> tokens" % (
+                    tuple(len(v) for v in vps), plan.region_counts))
+            m._region_projector()
+            m._region_side(split.img_pos.numel())
+            region = self._region_inputs([r for v in vps for r in v])
+        outs = m._prompts_forward(self, split, plan, region)
+        done = None
+        if m.device.type == "cuda":
+            done = torch.cuda.Event()
+            done.record(torch.cuda.current_stream(m.device))
         return PendingSeg(m, [(out, None, t) for out, t in zip(outs, things)], self.image_hw, self.seg_info[:1],
                           self.boxes[:1], done, (m.object_mask_threshold, m.overlap_threshold), mask_format)
 
@@ -140,14 +177,17 @@ def _content_key(t):
 
 
 # The device tensors a CUDA graph reads from a plan input of a phase (PSALM._phase), by plan type
-_GRAPH_TENSORS = {SEQ.SequencePlan: ("tok_ids", "img_pos", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool"),
+_GRAPH_TENSORS = {SEQ.SequencePlan: ("tok_ids", "img_pos", "seg_pos", "pad_pos", "attention_mask", "cls_pool", "refer_pool",
+                                      "region_pos"),
                   SEQ.PromptSplit: ("tok_ids", "img_pos")}
 
 
 def _plan_key(plan):
-    """The structure of a SequencePlan a captured graph is bound to (shapes and which optional rows exist)."""
-    return (plan.B, plan.T, plan.n_img, plan.any_padding, None if plan.cls_pool is None else tuple(plan.cls_pool.shape),
-            plan.refer_pool is not None, None if plan.pad_pos is None else int(plan.pad_pos.numel()))
+    """The structure of a SequencePlan a captured graph is bound to (shapes, which optional rows exist, and the regions
+    per row of a plan with <region> rows)."""
+    key = (plan.B, plan.T, plan.n_img, plan.any_padding, None if plan.cls_pool is None else tuple(plan.cls_pool.shape),
+           plan.refer_pool is not None, None if plan.pad_pos is None else int(plan.pad_pos.numel()))
+    return key if plan.region_counts is None else key + (tuple(plan.region_counts),)
 
 
 def attach_rle(results):
@@ -586,22 +626,35 @@ class PSALM:
         cache.length = split.P
         return cache
 
-    def _prompts_core(self, state, cache, plan):
+    def _prompts_core(self, state, cache, plan, region=None, image_hw=None):
         """Device work of K prompt suffixes (plan on device) against an opened image and its prefix cache (capturable).
-        Returns forward_core's dict for the K prompts (pred_masks [K,Q,H4*W4], ...) and the suffix hidden states."""
+        Returns forward_core's dict for the K prompts (pred_masks [K,Q,H4*W4], ...) and the suffix hidden states.
+        `region`: (bits, row_prefix, sample-point indices) of the R regions of the prompts (ImageSession._region_inputs),
+        pooled from the image's projector tokens; `image_hw` is the size the bits are at."""
+        from . import kernels
         img_tok = state["img_tok"]
-        embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok[:, :0], self.seg_query)
+        region_feat = None
+        if region is not None:
+            bits, prefix, sel = region
+            R, dev = sel.shape[0], sel.device
+            side = self._region_side(img_tok.shape[1])
+            pts = kernels.region_points_gather(bits, prefix, sel, torch.arange(R, dtype=torch.int32, device=dev), *image_hw)
+            region_feat = kernels.region_pool(img_tok.contiguous(), pts, torch.zeros(R, dtype=torch.int32, device=dev),
+                                              side, side)
+        embeds = SEQ.materialize_embeds(plan, self.model.embed_tokens, img_tok[:, :0], self.seg_query, region_feat)
         hidden = self.model.phi.forward_suffix(embeds, cache, plan.attention_mask if plan.any_padding else None)
-        seg_q, SEG_emb, cls_emb, _ = self._llm_heads(plan, hidden)
+        seg_q, SEG_emb, cls_emb, rows = self._llm_heads(plan, hidden)
+        region_emb = None if rows is None else list(torch.split(rows, list(plan.region_counts), 0))
         out = self.predictor.forward_tokens(None, state["ms_sizes"], None, state["mask_size"], seg_q, SEG_emb, cls_emb,
-                                            memory=state["mem"])
+                                            region_embedding_list=region_emb, memory=state["mem"])
         out["mask_size"] = state["mask_size"]
         out["hidden"], out["seg_query"] = hidden, seg_q
         return out
 
     def _cached_split(self, prompts, image_hw):
         """(host PromptSplit, device suffix plan) of a prompt set, cached by content like `_cached_plan`."""
-        key = (tuple(image_hw),) + tuple(tuple(_content_key(p.get(n)) for n in SEQ.PROMPT_KEYS) for p in prompts)
+        key = (tuple(image_hw),) + tuple(tuple(_content_key(p.get(n)) for n in SEQ.PROMPT_KEYS) + ("visual_prompts" in p,)
+                                         for p in prompts)
 
         def make():
             import dataclasses
@@ -621,18 +674,22 @@ class PSALM:
             h, w = (h + 1) // 2, (w + 1) // 2
         return ((h - 1) // 2 + 1) * ((w - 1) // 2 + 1)   # conv3x3 stride 2 pad 1 of the projector
 
-    def _prompts_forward(self, sess, split, plan):
-        """Run the prompt pass of a session and cut its output into one forward_core-style dict per prompt."""
+    def _prompts_forward(self, sess, split, plan, region=None):
+        """Run the prompt pass of a session and cut its output into one forward_core-style dict per prompt.  `region`: the
+        device inputs of the prompts' regions (ImageSession._region_inputs); the graph reads its own copies of them."""
         cache = sess.prefix_cache(split)
         out = self._phase("_prompt_graphs", (sess.lane, self.seg_task) + _plan_key(plan),
-                          lambda p: self._prompts_core(sess.state, cache, p), refresh=(plan,), reads=(sess.state, cache))
+                          lambda p, *reg: self._prompts_core(sess.state, cache, p, reg or None, sess.image_hw),
+                          refresh=(plan,) + tuple(region or ()), reads=(sess.state, cache))
         outs = []
         for k, ncls in enumerate(split.n_classes):
             cls = out["pred_class_name_logits"]
             seg = out["pred_SEG_logits"]
+            reg = out["pred_region_logits"]
             outs.append(dict(pred_masks=out["pred_masks"][k:k + 1], mask_size=out["mask_size"],
                              pred_class_name_logits=None if cls is None else cls[k:k + 1, :, :ncls].contiguous(),
-                             pred_SEG_logits=None if seg is None else seg[k:k + 1]))
+                             pred_SEG_logits=None if seg is None else seg[k:k + 1],
+                             pred_region_logits=None if reg is None else [reg[k]]))
         return outs
 
     # ---- input staging: overlap the upload of batch k+1 with the compute of batch k ----------------------
@@ -881,9 +938,10 @@ class PSALM:
                                                            self.test_topk_per_image, sig)
             if self.region_on:   # llava_phi.py:1457-1466
                 r["instances"] = PP.region_inference(out["pred_region_logits"][b].float(), mp, sig)
-                gt = info["instances"].gt_masks
-                gt = gt.tensor if hasattr(gt, "tensor") else gt
-                r["gt"] = PP.sem_seg_postprocess(gt.to(mp.device).float(), (oh, ow), height, width)
+                gt = getattr(info.get("instances"), "gt_masks", None)   # a session's image may come without them
+                if gt is not None:
+                    gt = gt.tensor if hasattr(gt, "tensor") else gt
+                    r["gt"] = PP.sem_seg_postprocess(gt.to(mp.device).float(), (oh, ow), height, width)
             results.append(r)
         return results
 

@@ -52,6 +52,95 @@ def draw_point_indices(counts, num_sample_point=NUM_SAMPLE_POINT):
     return torch.stack(out).to(torch.int32)
 
 
+# ---- visual prompts: clicks, scribbles, boxes and masks at the original image size (COCO-Interactive) ------------------
+# enhance_with_circles radius per kind (coco_instance_mapper.py:247-249); boxes and masks are resized as they are
+VISUAL_PROMPT_RADIUS = {"point": 10, "scribble": 5, "box": 0, "mask": 0}
+
+
+def _rle_has_foreground(counts):
+    """Whether a COCO compressed RLE string (rleFrString's LEB128-like code) has a non-zero run of ones."""
+    s = counts.encode("ascii") if isinstance(counts, str) else bytes(counts)
+    runs, p = [], 0
+    while p < len(s):
+        x, k, more = 0, 0, True
+        while more:
+            c = s[p] - 48
+            x |= (c & 0x1f) << (5 * k)
+            more = bool(c & 0x20)
+            p += 1
+            k += 1
+            if not more and c & 0x10:
+                x |= -1 << (5 * k)
+        if len(runs) > 2:
+            x += runs[-2]
+        runs.append(x)
+    return any(n > 0 for n in runs[1::2])
+
+
+def _source_masks(prompts, height, width, device):
+    """(uint8 [K,height,width] prompt masks on `device`, int32 [K] radii) of K (kind, source) pairs; ValueError for an
+    unknown kind, a source of the wrong form or size, or an empty source, before anything is launched."""
+    from . import rle
+    K = len(prompts)
+    if K == 0:
+        raise ValueError("visual_prompts: no regions")
+    src = torch.zeros((K, height, width), dtype=torch.uint8, device=device)
+    radius, rles = [], []
+    for k, p in enumerate(prompts):
+        if not isinstance(p, (tuple, list)) or len(p) != 2:
+            raise ValueError("visual prompt %d: expected a (kind, source) pair" % k)
+        kind, s = p
+        if kind not in VISUAL_PROMPT_RADIUS:
+            raise ValueError("visual prompt %d: kind %r is not one of %s" % (k, kind, sorted(VISUAL_PROMPT_RADIUS)))
+        r = VISUAL_PROMPT_RADIUS[kind]
+        radius.append(r)
+        if isinstance(s, dict):                    # COCO RLE at the original size
+            if [int(v) for v in s.get("size", ())] != [height, width]:
+                raise ValueError("visual prompt %d: RLE size %s, the image is %dx%d" % (k, s.get("size"), height, width))
+            if not isinstance(s.get("counts"), (str, bytes, bytearray)) or not _rle_has_foreground(s["counts"]):
+                raise ValueError("visual prompt %d: empty source mask" % k)
+            rles.append((k, s))
+        elif isinstance(s, torch.Tensor):          # binary [H0, W0], host or device
+            if tuple(s.shape) != (height, width):
+                raise ValueError("visual prompt %d: mask %s, the image is %dx%d" % (k, tuple(s.shape), height, width))
+            s = s.to(device).to(torch.uint8)       # binary_mask.astype(np.uint8) (:27)
+            if not bool((s == 1).any() if r > 0 else (s != 0).any()):   # only pixels equal to 1 seed a disk (:30)
+                raise ValueError("visual prompt %d: empty source mask" % k)
+            src[k] = s
+        elif kind == "point" and len(s) == 2:      # a click (row, col)
+            y, x = (int(v) for v in s)
+            if not (0 <= y < height and 0 <= x < width):
+                raise ValueError("visual prompt %d: point %s outside the %dx%d image" % (k, (y, x), height, width))
+            src[k, y, x] = 1
+        elif kind == "box" and len(s) == 4:        # (min_row, min_col, max_row, max_col), half-open (bulid_COCO_...:72)
+            y0, x0, y1, x1 = (int(v) for v in s)
+            y0, x0, y1, x1 = max(0, y0), max(0, x0), min(height, y1), min(width, x1)
+            if y1 <= y0 or x1 <= x0:
+                raise ValueError("visual prompt %d: empty source mask (box %s)" % (k, tuple(s)))
+            src[k, y0:y1, x0:x1] = 1
+        else:
+            raise ValueError("visual prompt %d: a %s takes an RLE dict, a [H, W] tensor%s" % (
+                k, kind, {"point": " or a (row, col) pixel", "box": " or (min_row, min_col, max_row, max_col)"}.get(kind, "")))
+    if rles:
+        dec = rle.decode([s for _, s in rles], device)
+        for i, (k, _) in enumerate(rles):
+            src[k] = dec[i]
+    return src, torch.tensor(radius, dtype=torch.int32).to(device)
+
+
+def rasterize_visual_prompts(prompts, height, width, resized_hw, padded_hw, device):
+    """K visual prompts (kind, source) of an image of original size (height, width) -> the region masks the reference
+    mapper gives (coco_instance_mapper.py:233-251: decode, enhance_with_circles for points and scribbles, NEAREST resize
+    to `resized_hw`, zero padding to `padded_hw`) as (bits, row_prefix, count) in the layout `region_points_gather`
+    reads, on `device`.  `kind` is "point", "scribble", "box" or "mask"; `source` is a COCO RLE dict at the original
+    size, a binary [height, width] tensor, a (row, col) pixel for a point or a (min_row, min_col, max_row, max_col) box."""
+    from . import kernels
+    from .image_processor import nearest_pad_tables
+    src, radius = _source_masks(prompts, int(height), int(width), device)
+    rows, cols = nearest_pad_tables(int(height), int(width), resized_hw, padded_hw)
+    return kernels.visual_prompt_raster(src, radius, rows.to(device), cols.to(device))
+
+
 def region_inputs(seg_info, region_points=None, attr="region_masks"):
     """seg_info: list of dicts with 'instances' (`.region_masks.tensor` [K,H,W], llava_phi.py:792; the DAVIS variant reads
     `.vp_region_masks`, :1664) -> (points [R,P,2] fp32, region_image [R] int32, counts).  `region_points`: optional

@@ -227,19 +227,27 @@ def split_prompts(prompts, n_img, n_q):
     """Cut K prompts of one image into the shared prefix and K suffixes (input_ids space).  The prefix is the longest
     common token prefix of the prompts, truncated at the first position that feeds an output (a <seg>, <cls>, <refer> or
     <region> sentinel, or a non-zero class-name / refer embedding index).  It must hold the <image> sentinel and no masked
-    position.  Raises ValueError (or NotImplementedError for <region> prompts) instead of falling back."""
+    position.  <region> prompts need their regions as `visual_prompts` (one (kind, source) pair per <region> token, see
+    ImageSession.eval_seg); the suffixes then carry region_pos / region_counts.  Raises ValueError (or
+    NotImplementedError for <region> prompts without visual_prompts) instead of falling back."""
     if not prompts:
         raise ValueError("no prompts")
+    if len({"visual_prompts" in p for p in prompts}) > 1:
+        raise ValueError("prompts of one call must all have or all lack visual_prompts")
     rows = []
     for k, p in enumerate(prompts):
-        unknown = set(p) - set(PROMPT_KEYS) - {"is_thing_list"}
+        unknown = set(p) - set(PROMPT_KEYS) - {"is_thing_list", "visual_prompts"}
         if unknown:
             raise ValueError("prompt %d: unknown keys %s" % (k, sorted(unknown)))
         r = {n: _row(p.get(n), n) for n in PROMPT_KEYS if n not in ("class_name_ids", "cls_indices", "token_refer_id")}
         r["ids"] = r.pop("input_ids").numpy().astype(np.int64)
-        if (r["ids"] == REGION_TOKEN_INDEX).any():
-            raise NotImplementedError("<region> prompts pool their features per prompt from sampled points; they are not "
-                                      "supported by multi-prompt sessions")
+        n_regions = int((r["ids"] == REGION_TOKEN_INDEX).sum())
+        if n_regions and "visual_prompts" not in p:
+            raise NotImplementedError("<region> prompts of a session need their regions as visual_prompts (the "
+                                      "per-image region_masks of eval_seg are not read by sessions)")
+        if "visual_prompts" in p and len(p["visual_prompts"]) != n_regions:
+            raise ValueError("prompt %d: %d visual prompts for %d <region> tokens" % (k, len(p["visual_prompts"]),
+                                                                                    n_regions))
         T0 = len(r["ids"])
         r["am"] = np.ones(T0, bool) if r["attention_mask"] is None else r["attention_mask"].numpy().astype(bool)
         r["cei"] = None if r["class_name_embedding_indices"] is None else r["class_name_embedding_indices"].numpy()
