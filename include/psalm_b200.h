@@ -75,16 +75,7 @@ int psalm_msda_forward(const void* value, const int64_t* shapes, const int64_t* 
  *          dtype ow_dtype (F32 / F16 / BF16).  Lq must equal S (encoder self-attention).
  *   out    [B,Lq,M*D] dtype value_dtype
  *   shapes_host/starts_host: HOST int64 arrays.
- * Three kernels sit behind the call (psalm_set_msda_impl: 0 = auto (= 1), 1, 2, 3):
- *   1  one lane group per (query, head), corners gathered from global memory / L1 (measured fastest);
- *   2  paired columns (the two x-adjacent bilinear corners are one contiguous access);
- *   3  (16-bit storage, M=8, D=32, L=3, P=4, levels ordered coarse to fine) value tiles of a 16x16 cell of the finest
- *      level (+ halo) staged in shared memory by TMA (cp.async.bulk.tensor.4d, zero fill = the op's zero padding), the
- *      gather + weighted sum as ldmatrix gathers + mma.sync (csrc/msda_smem.cu); samples beyond the halo
- *      (psalm_set_msda_halo, default 5 pixels) read global memory - results do not depend on the halo.  Correct,
- *      selectable, measured slower than 1 (DESIGN.md section 5). */
-int psalm_set_msda_impl(int impl);
-int psalm_set_msda_halo(int halo);
+ * One kernel sits behind the call: one lane group per (query, head), corners gathered from global memory / L1. */
 int psalm_msda_encoder_fused(const void* value, const void* ow, void* out,
                              const int64_t* shapes_host, const int64_t* starts_host,
                              int B, int S, int M, int D, int L, int P,

@@ -44,8 +44,6 @@ SIGNATURES = {
     "psalm_bilinear_tokens": ([_c_vp] * 2 + [_c_i] * 9 + [_c_vp], _c_i),
     "psalm_attn_mask_bits": ([_c_vp] * 3 + [_c_i] * 3 + [_c_vp], _c_i),
     "psalm_set_postproc_impl": ([_c_i], _c_i),
-    "psalm_set_msda_impl": ([_c_i], _c_i),
-    "psalm_set_msda_halo": ([_c_i], _c_i),
     "psalm_set_causal_impl": ([_c_i], _c_i),
     "psalm_postproc_partials": ([_c_i] * 8 + [ctypes.POINTER(_c_i)], _c_i),
     "psalm_postproc_fused": ([_c_vp] * 10 + [_c_i] * 8 + [_c_vp], _c_i),

@@ -470,142 +470,6 @@ static int launch_msda(const void* value, const int64_t* shapes, const int64_t* 
   return check_launch("msda_vec_kernel");
 }
 
-
-// -------------------------------------------------------------------------------------------
-// Paired-column variant of the fused kernel: a (query, head) pair is owned by 2*G lanes.  Lanes 0..G-1 fetch the
-// x0 column of every bilinear sample, lanes G..2G-1 the x1 column, so the two x-adjacent corners (adjacent
-// 16*G-byte pixel records of the head-major value plane) are ONE 32*G-byte access per row instead of two separate
-// instructions: a single L1 wavefront whenever x0 is even, i.e. ~25 % fewer wavefronts on the L1 gather path
-// (DESIGN.md section 5).  Each half keeps partial sums; one xor-shuffle merges them at the end.
-// Measured SLOWER than the single-group kernel (59.4 vs 53.4 us cold-cache at 1024^2, bf16): half as many queries
-// per CTA and the softmax / sample arithmetic done twice cost more than the saved wavefronts.  Kept selectable
-// (psalm_set_msda_impl(2)) and tested, not used by default.
-// -------------------------------------------------------------------------------------------
-template <typename TV, typename TO, int G, int LT, int PT>
-__global__ void __launch_bounds__(kThreads)
-msda_encoder_fused_pair_kernel(const TV* __restrict__ value, const TO* __restrict__ ow,
-                               TV* __restrict__ out, MsdaLevels lv, int S, int M, int D) {
-  constexpr int CH = 16 / sizeof(TV);
-  constexpr int GG = 2 * G;
-  constexpr int NG = kThreads / GG;
-  constexpr int LP = LT * PT;
-  constexpr int SPL = (LP + G - 1) / G;   // samples owned per lane (within its half)
-  const int g = threadIdx.x / GG, cl = threadIdx.x % G, half = (threadIdx.x / G) & 1;
-  const int lane = threadIdx.x & 31;
-  const int hbase = lane - cl;            // first lane of this half-group inside the warp
-  const int m = blockIdx.y, b = blockIdx.z;
-  int q, ql, qy, qx;
-  const bool active = resolve_query<NG>(lv, true, g, S, q, ql, qy, qx);
-  if (!active) {
-    q = lv.start[ql];
-    qy = qx = 0;
-  }
-  const size_t row = ((size_t)b * S + q) * (size_t)(M * LP * 3);
-  const TO* __restrict__ offp = ow + row + (size_t)m * LP * 2;
-  const TO* __restrict__ lgp = ow + row + (size_t)M * LP * 2 + (size_t)m * LP;
-
-  // softmax over the L*P logits, computed redundantly by both halves (G lanes each)
-  float lg[SPL];
-  float mx = -INFINITY;
-#pragma unroll
-  for (int j = 0; j < SPL; ++j) {
-    const int s = cl + j * G;
-    lg[j] = s < LP ? to_f32<TO>(lgp[s]) : -INFINITY;
-    mx = fmaxf(mx, lg[j]);
-  }
-#pragma unroll
-  for (int o = 1; o < G; o <<= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  float sum = 0.f;
-#pragma unroll
-  for (int j = 0; j < SPL; ++j) {
-    lg[j] = (cl + j * G) < LP ? expf(lg[j] - mx) : 0.f;
-    sum += lg[j];
-  }
-#pragma unroll
-  for (int o = 1; o < G; o <<= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float inv = 1.f / sum;
-
-  const float rx = ((float)qx + 0.5f) / (float)lv.W[ql];
-  const float ry = ((float)qy + 0.5f) / (float)lv.H[ql];
-
-  // parameters of the samples this lane owns, for ITS column: top / bottom corner offsets and weights
-  constexpr int DC = G * CH;
-  uint32_t poff[SPL][2];
-  float pw[SPL][2];
-#pragma unroll
-  for (int j = 0; j < SPL; ++j) {
-    const int s = cl + j * G;
-    poff[j][0] = poff[j][1] = 0u;
-    pw[j][0] = pw[j][1] = 0.f;
-    if (s < LP) {
-      const int l = s / PT;
-      const int H = lv.H[l], W = lv.W[l];
-      float ox, oy;
-      if constexpr (sizeof(TO) == 4) {
-        const float2 o2 = __ldg(reinterpret_cast<const float2*>(offp) + s);
-        ox = o2.x; oy = o2.y;
-      } else {
-        unpack2<TO>(__ldg(reinterpret_cast<const uint32_t*>(offp) + s), ox, oy);
-      }
-      const float x = (rx + ox / (float)W) * (float)W - 0.5f;
-      const float y = (ry + oy / (float)H) * (float)H - 0.5f;
-      if (y > -1.f && x > -1.f && y < (float)H && x < (float)W) {
-        const float yf = floorf(y), xf = floorf(x);
-        const int y0 = (int)yf, x0 = (int)xf;
-        const float ly = y - yf, lx = x - xf, hy = 1.f - ly, hx = 1.f - lx;
-        const float aw = lg[j] * inv;
-        const bool vy0 = y0 >= 0, vy1 = y0 + 1 <= H - 1;
-        const bool vx = half ? (x0 + 1 <= W - 1) : (x0 >= 0);        // this half's column exists
-        const float wx = (half ? lx : hx) * aw;
-        pw[j][0] = (vy0 && vx) ? hy * wx : 0.f;
-        pw[j][1] = (vy1 && vx) ? ly * wx : 0.f;
-        const int y0c = y0 < 0 ? 0 : y0, y1c = y0 + 1 > H - 1 ? H - 1 : y0 + 1;
-        int xc = x0 + half;
-        xc = xc < 0 ? 0 : (xc > W - 1 ? W - 1 : xc);
-        const int st = lv.start[l];
-        poff[j][0] = (uint32_t)((st + y0c * W + xc) * DC);
-        poff[j][1] = (uint32_t)((st + y1c * W + xc) * DC);
-      }
-    }
-  }
-
-  const TV* __restrict__ vb = value + ((size_t)b * M + m) * (size_t)S * DC + cl * CH;
-  float2 acc2[CH / 2];
-#pragma unroll
-  for (int i = 0; i < CH / 2; ++i) acc2[i] = make_float2(0.f, 0.f);
-
-#pragma unroll
-  for (int s = 0; s < LP; ++s) {
-    const int owner = hbase + (s % G), j = s / G;
-    const uint32_t o0 = __shfl_sync(0xffffffffu, poff[j][0], owner);
-    const uint32_t o1 = __shfl_sync(0xffffffffu, poff[j][1], owner);
-    const float w0 = __shfl_sync(0xffffffffu, pw[j][0], owner);
-    const float w1 = __shfl_sync(0xffffffffu, pw[j][1], owner);
-    float2 f0[CH / 2], f1[CH / 2];
-    load16_as_f32x2<TV>(vb + o0, f0);
-    load16_as_f32x2<TV>(vb + o1, f1);
-#pragma unroll
-    for (int i = 0; i < CH / 2; ++i) {
-      ffma2(acc2[i], f0[i], w0);
-      ffma2(acc2[i], f1[i], w1);
-    }
-  }
-  float acc[CH];
-#pragma unroll
-  for (int i = 0; i < CH / 2; ++i) {   // x0 column + x1 column
-    acc[2 * i] = acc2[i].x + __shfl_xor_sync(0xffffffffu, acc2[i].x, G);
-    acc[2 * i + 1] = acc2[i].y + __shfl_xor_sync(0xffffffffu, acc2[i].y, G);
-  }
-  if (active && half == 0) store16_from_f32<TV>(out + (((size_t)b * S + q) * M + m) * (size_t)DC + cl * CH, acc);
-}
-
-int g_msda_fused_impl = 0;   // 0 auto, 1 one lane group per (query, head), 2 paired columns, 3 TMA-staged tiles + mma (msda_smem.cu)
-
-// TMA-staged shared-memory tiles + tensor-core contraction (msda_smem.cu): 16-bit storage, M = 8, D = 32, L = 3, P = 4
-bool msda_smem_ok(int M, int D, int L, int P, int value_dtype, const int64_t* shapes_host);
-int msda_smem_fused(const void* value, const void* ow, void* out, const int64_t* shapes_host, const int64_t* starts_host, int B,
-                    int S, int value_dtype, int ow_dtype, cudaStream_t st);
-
 template <typename TV, typename TO>
 static int launch_fused(const void* value, const void* ow, void* out, const int64_t* shapes_host,
                         const int64_t* starts_host, int B, int S, int M, int D, int L, int P,
@@ -616,22 +480,16 @@ static int launch_fused(const void* value, const void* ow, void* out, const int6
   PSALM_REQUIRE(G == 4 || G == 8, "msda_fused: D=%d unsupported (need D/%d in {4,8})", D, CH);
   PSALM_REQUIRE((long long)S * D < (1ll << 31), "msda_fused: S*D=%lld exceeds the 32-bit corner offsets", (long long)S * D);
   PSALM_REQUIRE((L == 3 || L == 4) && P == 4, "msda_fused: (L,P)=(%d,%d) unsupported", L, P);
-  const bool pair = g_msda_fused_impl == 2 && 2 * G <= 32;
   MsdaLevels lv;
   int tiles = 0;
   long long sumHW = 0;
-  fill_levels(lv, shapes_host, starts_host, L, kThreads / (pair ? 2 * G : G), tiles, sumHW);
+  fill_levels(lv, shapes_host, starts_host, L, kThreads / G, tiles, sumHW);
   PSALM_REQUIRE(sumHW == S, "msda_fused: sum(H_l*W_l)=%lld != S=%d", sumHW, S);
   dim3 grid(tiles, M, B);
-#define PSALM_FUSED(KERN, GG, LT)                                                                   \
-  KERN<TV, TO, GG, LT, 4><<<grid, kThreads, 0, st>>>((const TV*)value, (const TO*)ow, (TV*)out, lv, S, M, D)
-  if (pair) {
-    if (G == 4) { if (L == 3) PSALM_FUSED(msda_encoder_fused_pair_kernel, 4, 3); else PSALM_FUSED(msda_encoder_fused_pair_kernel, 4, 4); }
-    else        { if (L == 3) PSALM_FUSED(msda_encoder_fused_pair_kernel, 8, 3); else PSALM_FUSED(msda_encoder_fused_pair_kernel, 8, 4); }
-  } else {
-    if (G == 4) { if (L == 3) PSALM_FUSED(msda_encoder_fused_kernel, 4, 3); else PSALM_FUSED(msda_encoder_fused_kernel, 4, 4); }
-    else        { if (L == 3) PSALM_FUSED(msda_encoder_fused_kernel, 8, 3); else PSALM_FUSED(msda_encoder_fused_kernel, 8, 4); }
-  }
+#define PSALM_FUSED(GG, LT)                                                                         \
+  msda_encoder_fused_kernel<TV, TO, GG, LT, 4><<<grid, kThreads, 0, st>>>((const TV*)value, (const TO*)ow, (TV*)out, lv, S, M, D)
+  if (G == 4) { if (L == 3) PSALM_FUSED(4, 3); else PSALM_FUSED(4, 4); }
+  else        { if (L == 3) PSALM_FUSED(8, 3); else PSALM_FUSED(8, 4); }
 #undef PSALM_FUSED
   return check_launch("msda_encoder_fused_kernel");
 }
@@ -666,12 +524,10 @@ extern "C" int psalm_msda_forward(const void* value, const int64_t* shapes, cons
   return PSALM_E_ARG;
 }
 
-extern "C" int psalm_set_msda_impl(int impl) {
-  PSALM_REQUIRE(impl >= 0 && impl <= 3, "set_msda_impl: 0 (auto), 1 (one lane group per query-head), 2 (paired columns) or 3 (TMA tiles)");
-  psalm::g_msda_fused_impl = impl;
-  return PSALM_OK;
-}
-
+// Two alternatives to msda_encoder_fused_kernel were tried and measured slower at 1024^2 (bf16, per layer-image):
+// paired columns (2*G lanes per (query, head), the two x-adjacent corners as one access), 59.4 vs 53.4 us, and
+// value tiles staged in shared memory by TMA with the weighted sum on mma.sync, 84 vs 53 us (53.7 M vs 39 M warp
+// instructions).
 extern "C" int psalm_msda_encoder_fused(const void* value, const void* ow, void* out,
                                         const int64_t* shapes_host, const int64_t* starts_host, int B,
                                         int S, int M, int D, int L, int P, int value_dtype, int ow_dtype,
@@ -679,18 +535,6 @@ extern "C" int psalm_msda_encoder_fused(const void* value, const void* ow, void*
   PSALM_REQUIRE(value && ow && out && shapes_host && starts_host, "msda_fused: null pointer argument");
   PSALM_REQUIRE(B > 0 && S > 0 && M > 0 && D > 0, "msda_fused: non-positive dimension");
   cudaStream_t st = (cudaStream_t)stream;
-  // auto = the L1-gather kernel: the TMA-tile + mma kernel (impl 3) is correct but measured slower at 1024^2
-  // (84 us vs 53 us per layer-image: 53.7 M vs 39 M warp instructions, DESIGN.md section 5)
-  if (g_msda_fused_impl == 3) {
-    const bool ok = msda_smem_ok(M, D, L, P, value_dtype, shapes_host) && M <= 65535 && B <= 65535;
-    if (ok) {
-      long long sum = 0;
-      for (int l = 0; l < L; ++l) sum += shapes_host[2 * l] * shapes_host[2 * l + 1];
-      PSALM_REQUIRE(sum == S, "msda_fused: sum(H_l*W_l)=%lld != S=%d", sum, S);
-      return msda_smem_fused(value, ow, out, shapes_host, starts_host, B, S, value_dtype, ow_dtype, st);
-    }
-    PSALM_REQUIRE(false, "msda_fused: the TMA-tile kernel needs 16-bit storage, M=8, D=32, L=3, P=4, levels coarse to fine");
-  }
 #define ARGS value, ow, out, shapes_host, starts_host, B, S, M, D, L, P, st
   if (value_dtype == PSALM_F32 && ow_dtype == PSALM_F32) return launch_fused<float, float>(ARGS);
   if (value_dtype == PSALM_F16 && ow_dtype == PSALM_F16) return launch_fused<__half, __half>(ARGS);

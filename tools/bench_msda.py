@@ -92,12 +92,8 @@ def main():
             for odt, oname in ((dt, name), (torch.float32, "f32")):
                 ow = torch.cat([off.reshape(B, S, -1), logits.reshape(B, S, -1)], -1).to(odt).contiguous()
                 bytes_fused = B * (es * S * M * D * 2 + ow.element_size() * S * M * L * P * 3)
-                from psalm_b200 import _lib
-                for impl, iname in ((1, "single"), (2, "paired")) + (((3, "tma_tiles"),) if dt != torch.float32 else ()):
-                    _lib.check(_lib.lib().psalm_set_msda_impl(impl), "set_msda_impl")
-                    med, best = timeit(lambda: msda.msda_encoder_fused(vh, ow, shapes, st, P), flush=flush)
-                    res["%s_fused_%s_ow%s_spread%g" % (name, iname, oname, spread)] = dict(us=med, best_us=best, gbs=bytes_fused / med / 1e3, frac=bytes_fused / med / 1e3 / hbm)
-                _lib.lib().psalm_set_msda_impl(0)
+                med, best = timeit(lambda: msda.msda_encoder_fused(vh, ow, shapes, st, P), flush=flush)
+                res["%s_fused_ow%s_spread%g" % (name, oname, spread)] = dict(us=med, best_us=best, gbs=bytes_fused / med / 1e3, frac=bytes_fused / med / 1e3 / hbm)
     for k, v in res.items():
         print("%-40s %8.1f us (best %7.1f)  %8.1f GB/s  frac %.3f" % (k, v["us"], v["best_us"], v["gbs"], v.get("frac", 0)))
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
