@@ -182,7 +182,9 @@ int psalm_add_layernorm(const void* x, const void* r1, const void* r2, const voi
  * msdeformattn.py:199-203,244-252.  Deterministic (no atomics).
  * pre_bias [C] or NULL: per-channel bias of the conv / Linear that produced x, added before the statistics
  * (GroupNorm(x + pre_bias)): the producer runs without its separate broadcast bias-add pass.
- * stats_workspace: at least 8 * B * groups * (1 + ceil(N / 256)) bytes. */
+ * stats_workspace: 16-byte aligned, at least 8 * (2 * ceil(B * groups / 2) + 2 * ceil(B * groups * S / 2)
+ * + 2 * B * groups * S) bytes with S = ceil(N / 256): fp32 (mean, rstd) per (batch, group), then per (batch, group,
+ * 256-token slice) the fp32 raw moments and the double centred (mean, M2). */
 int psalm_groupnorm_tokens(const void* x, const void* pre_bias, const void* weight, const void* bias, void* y,
                            double* stats_workspace, int B, int N, int C, int groups, float eps, int relu,
                            int dtype, void* stream);

@@ -5,8 +5,9 @@
 //                   input_layernorm), the encoder / decoder post-norm layers (msdeformattn.py:59-65,
 //                   mask2former_transformer_decoder.py:42-43,102-103,160-161).  One warp per row,
 //                   the row lives in registers (two-pass mean / variance like ATen), 16-byte accesses.
-//   groupnorm_tokens  GroupNorm(32) on a TOKEN-MAJOR map [B, N, C] (+ optional ReLU): deterministic
-//                   per-CTA partial sums -> fixed-order finalize (double) -> streaming apply pass (msdeformattn.py:199-203,244-252 conv+GN(+ReLU) blocks).
+//   groupnorm_tokens  GroupNorm(32) on a TOKEN-MAJOR map [B, N, C] (+ optional ReLU): deterministic per-CTA raw and
+//                   centred moments of each slice -> fixed-order combine (double) -> streaming apply pass
+//                   (msdeformattn.py:199-203,244-252 conv+GN(+ReLU) blocks).
 #include "common.cuh"
 
 namespace psalm {
@@ -169,35 +170,53 @@ static int launch_pm(const void* x, const void* w, const void* b, void* y, int B
 }
 
 // ---- GroupNorm on token-major maps -----------------------------------------------------------------
-// Deterministic (no atomics): (1) per-CTA partial (sum, sumsq) per group over a slice of 256 tokens,
-// reduced inside the CTA in a fixed order; (2) a finalize kernel adds the partials of each (batch, group)
-// in a fixed order in double and emits (mean, rstd); (3) streaming apply.
+// Deterministic (no atomics), and free of cancellation when |mean| >> std:
+// (1) groupnorm_partial_kernel, one CTA per (slice of GN_TOKENS tokens, batch).  Pass 1 sums x and x^2 of each group in
+//     fp32 (one chain per thread over its tokens and 4 channels, then the thread sums of a group in a fixed order): the
+//     raw moments.  Their slice mean m~ is the pivot of pass 2, which re-reads the slice (L1 / L2 resident) and sums
+//     d = x - m~ and d^2 with two accumulators per channel; the CTA emits in double the slice's centred
+//     (mean, M2) = (m~ + S_d / n, S_dd - S_d^2 / n), whose rounding scales with the spread of the group, not its offset.
+// (2) groupnorm_finalize_kernel, one warp per (batch, group), combines the slices in a fixed order in double: the raw
+//     moments in slice order into E[x], E[x^2] - E[x]^2, and the centred ones with Chan et al.'s formula
+//     (mean = sum n_k mean_k / n, M2 = sum M2_k + n_k (mean_k - mean)^2).  Where the raw statistics agree with the
+//     centred ones to GN_AGREE (mean within GN_AGREE * sqrt(var + eps), var within GN_AGREE * (var + eps)) they are
+//     used, so that well-conditioned groups keep exactly the statistics of the raw-moment formula; otherwise (an offset
+//     that has cancelled the raw variance) the centred ones.  rstd = rsqrtf(var + eps).
+// (3) groupnorm_apply_kernel streams y = (x + pre_bias - mean) * rstd * w + b (+ ReLU).
 // C <= 1024, C % (4*groups) == 0, 256 % (C/4) == 0.
+constexpr int GN_TOKENS = 256;
+constexpr double GN_AGREE = 1.0 / 524288;   // 2^-19
+
 template <typename T>
 __global__ void __launch_bounds__(256) groupnorm_partial_kernel(const T* __restrict__ x, const T* __restrict__ pre_bias,
-                                                                float2* __restrict__ part,
-                                                                int N, int C, int groups, int tokens_per_cta) {
-  __shared__ float ts[256], tq[256];
-  const int b = blockIdx.y;
-  const int t0 = blockIdx.x * tokens_per_cta;
-  const int t1 = min(N, t0 + tokens_per_cta);
+                                                                float2* __restrict__ raw, double2* __restrict__ part, int N,
+                                                                int C, int groups) {
+  __shared__ float ts[256], tq[256], piv[64];
   const int cpg = C / groups;
   const int chunks = C / 4;                    // 4-element chunks per token
-  const int tpb = 256 / chunks;                // tokens processed concurrently
+  const int tpb = 256 / chunks;                // tokens processed concurrently (every thread has a chunk)
+  const int cpgc = cpg / 4;                    // chunks per group
   const int cidx = threadIdx.x % chunks, trow = threadIdx.x / chunks;
+  const int b = blockIdx.y;
+  const int t0 = blockIdx.x * GN_TOKENS;
+  const int t1 = min(N, t0 + GN_TOKENS);
+  const T* xb = x + (size_t)b * N * C + cidx * 4;
+  float pb[4] = {0.f, 0.f, 0.f, 0.f};          // per-channel bias of the producing conv / linear, folded in here
+  if (pre_bias) load4<T>(pre_bias + cidx * 4, pb);
+  const size_t slot = ((size_t)b * groups + threadIdx.x) * gridDim.x + blockIdx.x;
+  const double n = (double)(t1 - t0) * cpg;    // values of one group in this slice
+
+  // pass 1: raw moments
   float s = 0.f, q = 0.f;
-  if (trow < tpb) {
-    float pb[4] = {0.f, 0.f, 0.f, 0.f};        // per-channel bias of the producing conv / linear, folded in here
-    if (pre_bias) load4<T>(pre_bias + cidx * 4, pb);
-    for (int t = t0 + trow; t < t1; t += tpb) {
-      float f[4];
-      load4<T>(x + ((size_t)b * N + t) * C + cidx * 4, f);
+#pragma unroll 4
+  for (int t = t0 + trow; t < t1; t += tpb) {
+    float f[4];
+    load4<T>(xb + (size_t)t * C, f);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        f[i] += pb[i];
-        s += f[i];
-        q = fmaf(f[i], f[i], q);
-      }
+    for (int i = 0; i < 4; ++i) {
+      f[i] += pb[i];
+      s += f[i];
+      q = fmaf(f[i], f[i], q);
     }
   }
   ts[threadIdx.x] = s;
@@ -205,7 +224,6 @@ __global__ void __launch_bounds__(256) groupnorm_partial_kernel(const T* __restr
   __syncthreads();
   if (threadIdx.x < groups) {
     const int g = threadIdx.x;
-    const int cpgc = cpg / 4;                  // chunks per group
     float gs = 0.f, gq = 0.f;
     for (int r = 0; r < tpb; ++r)
       for (int c = 0; c < cpgc; ++c) {
@@ -213,24 +231,90 @@ __global__ void __launch_bounds__(256) groupnorm_partial_kernel(const T* __restr
         gs += ts[t];
         gq += tq[t];
       }
-    part[((size_t)b * groups + g) * gridDim.x + blockIdx.x] = make_float2(gs, gq);
+    raw[slot] = make_float2(gs, gq);
+    piv[g] = (float)((double)gs / n);
+  }
+  __syncthreads();
+
+  // pass 2: centred sums around the slice mean, two accumulators per channel (even / odd tokens of the thread)
+  const float m = piv[cidx / cpgc];
+  float d1[2][4] = {}, d2[2][4] = {};
+#pragma unroll 2
+  for (int t = t0 + trow; t < t1; t += 2 * tpb) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (t + h * tpb < t1) {
+        float f[4];
+        load4<T>(xb + (size_t)(t + h * tpb) * C, f);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float d = (f[i] + pb[i]) - m;
+          d1[h][i] += d;
+          d2[h][i] = fmaf(d, d, d2[h][i]);
+        }
+      }
+    }
+  }
+  float e1[4], e2[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    e1[i] = d1[0][i] + d1[1][i];
+    e2[i] = d2[0][i] + d2[1][i];
+  }
+  ts[threadIdx.x] = (e1[0] + e1[1]) + (e1[2] + e1[3]);
+  tq[threadIdx.x] = (e2[0] + e2[1]) + (e2[2] + e2[3]);
+  __syncthreads();
+  if (threadIdx.x < groups) {
+    const int g = threadIdx.x;
+    float gs = 0.f, gq = 0.f;
+    for (int r = 0; r < tpb; ++r)
+      for (int c = 0; c < cpgc; ++c) {
+        const int t = r * chunks + g * cpgc + c;
+        gs += ts[t];
+        gq += tq[t];
+      }
+    const double sd = gs;
+    part[slot] = make_double2((double)piv[g] + sd / n, (double)gq - sd * sd / n);
   }
 }
 
-__global__ void groupnorm_finalize_kernel(const float2* __restrict__ part, float2* __restrict__ mean_rstd, int n_bg,
-                                          int n_part, double count, float eps) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void groupnorm_finalize_kernel(const float2* __restrict__ raw, const double2* __restrict__ part,
+                                          float2* __restrict__ mean_rstd, int n_bg, int n_part, int N, int cpg, float eps) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (i >= n_bg) return;
-  double s = 0.0, q = 0.0;
-  for (int k = 0; k < n_part; ++k) {
-    const float2 v = part[(size_t)i * n_part + k];
-    s += (double)v.x;
-    q += (double)v.y;
+  const double2* p = part + (size_t)i * n_part;
+  const double full = (double)GN_TOKENS * cpg, last = (double)(N - (n_part - 1) * GN_TOKENS) * cpg;   // values per slice
+  const double n = (double)N * cpg;
+  // centred: lane l takes slices l, l + 32, ..., then a butterfly (fixed order)
+  double sm = 0.0;
+  for (int k = lane; k < n_part; k += 32) sm += (k + 1 < n_part ? full : last) * p[k].x;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sm += __shfl_xor_sync(0xffffffffu, sm, o);
+  const double mean = sm / n;
+  double m2 = 0.0;
+  for (int k = lane; k < n_part; k += 32) {
+    const double dk = p[k].x - mean;
+    m2 += p[k].y + (k + 1 < n_part ? full : last) * dk * dk;
   }
-  const double m = s / count;
-  double var = q / count - m * m;
-  if (var < 0) var = 0;
-  mean_rstd[i] = make_float2((float)m, rsqrtf((float)var + eps));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m2 += __shfl_xor_sync(0xffffffffu, m2, o);
+  if (lane == 0) {
+    const double var = m2 > 0.0 ? m2 / n : 0.0;
+    // raw moments, added in slice order
+    double s = 0.0, q = 0.0;
+    for (int k = 0; k < n_part; ++k) {
+      const float2 v = raw[(size_t)i * n_part + k];
+      s += (double)v.x;
+      q += (double)v.y;
+    }
+    const double m_raw = s / n;
+    double var_raw = q / n - m_raw * m_raw;
+    if (var_raw < 0) var_raw = 0;
+    const double ve = var + (double)eps;
+    const bool agree = fabs(m_raw - mean) <= GN_AGREE * sqrt(ve) && fabs(var_raw - var) <= GN_AGREE * ve;
+    const double mu = agree ? m_raw : mean, v = agree ? var_raw : var;
+    mean_rstd[i] = make_float2((float)mu, rsqrtf((float)v + eps));
+  }
 }
 
 template <typename T>
@@ -281,15 +365,15 @@ static int launch_ln(const void* x, const void* r1, const void* r2, const void* 
 template <typename T>
 static int launch_gn(const void* x, const void* pre_bias, const void* w, const void* b, void* y, double* workspace, int B, int N, int C,
                      int groups, float eps, int relu, cudaStream_t st) {
-  const int tokens_per_cta = 256;
-  const int n_part = (N + tokens_per_cta - 1) / tokens_per_cta;
+  const int n_part = (N + GN_TOKENS - 1) / GN_TOKENS;
+  const size_t n_bg = (size_t)B * groups;
+  const size_t n_raw = (n_bg * n_part + 1) & ~(size_t)1;                       // float2 = one double each
   float2* mean_rstd = reinterpret_cast<float2*>(workspace);                    // [B*groups]
-  float2* part = mean_rstd + (size_t)B * groups;                               // [B*groups][n_part]
+  float2* raw = reinterpret_cast<float2*>(workspace + ((n_bg + 1) & ~(size_t)1));          // [B*groups][n_part]
+  double2* part = reinterpret_cast<double2*>(workspace + ((n_bg + 1) & ~(size_t)1) + n_raw); // [B*groups][n_part], 16-B aligned
   dim3 g1(n_part, B);
-  groupnorm_partial_kernel<T><<<g1, 256, 0, st>>>((const T*)x, (const T*)pre_bias, part, N, C, groups, tokens_per_cta);
-  const int n_bg = B * groups;
-  groupnorm_finalize_kernel<<<(n_bg + 127) / 128, 128, 0, st>>>(part, mean_rstd, n_bg, n_part,
-                                                              (double)N * (C / groups), eps);
+  groupnorm_partial_kernel<T><<<g1, 256, 0, st>>>((const T*)x, (const T*)pre_bias, raw, part, N, C, groups);
+  groupnorm_finalize_kernel<<<(unsigned)((n_bg + 3) / 4), 128, 0, st>>>(raw, part, mean_rstd, (int)n_bg, n_part, N, C / groups, eps);
   const long long n4 = (long long)B * N * C / 4;
   const int blocks = (int)((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   groupnorm_apply_kernel<T><<<blocks > 0 ? blocks : 1, 256, 0, st>>>((const T*)x, (const T*)pre_bias, mean_rstd, (const T*)w, (const T*)b,
@@ -320,6 +404,8 @@ extern "C" int psalm_groupnorm_tokens(const void* x, const void* pre_bias, const
                                       double* stats_workspace, int B, int N, int C, int groups, float eps,
                                       int relu, int dtype, void* stream) {
   PSALM_REQUIRE(x && weight && bias && y && stats_workspace, "groupnorm_tokens: null pointer");
+  PSALM_REQUIRE(B > 0 && N > 0 && (reinterpret_cast<uintptr_t>(stats_workspace) & 15) == 0,
+                "groupnorm_tokens: B, N must be positive and the workspace 16-byte aligned");
   PSALM_REQUIRE(groups > 0 && groups <= 64 && C % (4 * groups) == 0 && C <= 1024 && 256 % (C / 4) == 0,
                 "groupnorm_tokens: unsupported C=%d groups=%d", C, groups);
   cudaStream_t st = (cudaStream_t)stream;

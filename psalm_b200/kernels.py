@@ -260,7 +260,10 @@ def group_norm_tokens(x, weight, bias, groups=32, eps=1e-5, relu=False, pre_bias
     for t, n in ((x, "x"), (weight, "weight"), (bias, "bias")) + (((pre_bias, "pre_bias"),) if pre_bias is not None else ()):
         _chk(t, "group_norm_tokens." + n)
     B, N, C = x.shape
-    stats = torch.empty(B * groups * (1 + (N + 255) // 256), dtype=torch.float64, device=x.device)
+    # (mean, rstd) per (batch, group), then per (batch, group, 256-token slice) the fp32 raw moments and the double
+    # centred (mean, M2); each region rounded up to 16 bytes
+    nbg, slices = B * groups, (N + 255) // 256
+    stats = torch.empty((nbg + 1) // 2 * 2 + (nbg * slices + 1) // 2 * 2 + 2 * nbg * slices, dtype=torch.float64, device=x.device)
     y = torch.empty_like(x)
     rc = _lib.lib().psalm_groupnorm_tokens(_lib.ptr(x), _lib.ptr(pre_bias) if pre_bias is not None else None,
                                            _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(y), _lib.ptr(stats),
