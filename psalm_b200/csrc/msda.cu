@@ -420,6 +420,9 @@ static int launch_msda(const void* value, const int64_t* shapes, const int64_t* 
                       ((L * P * 2 * sizeof(TL)) % 8 == 0) &&
                       ((reinterpret_cast<uintptr_t>(value) | reinterpret_cast<uintptr_t>(out)) % 16 == 0) &&
                       (reinterpret_cast<uintptr_t>(loc) % 8 == 0) && (reinterpret_cast<uintptr_t>(w) % 4 == 0);
+  // the (3,4) / (4,4) instantiations preload fp32 loc / w with float4 loads; a contiguous tensor with a storage offset
+  // can be 8-byte (loc) or 4-byte (w) aligned only, and then takes the runtime-(L,P) instantiation (float2 / scalar loads)
+  const bool preload_ok = sizeof(TL) != 4 || ((reinterpret_cast<uintptr_t>(loc) | reinterpret_cast<uintptr_t>(w)) % 16 == 0);
   const int G = vec_ok ? D / CH : 1;
   const int NG = kThreads / (G < 1 ? 1 : G);
   int tiles = 0;
@@ -451,9 +454,9 @@ static int launch_msda(const void* value, const int64_t* shapes, const int64_t* 
       pix_stride, head_stride, batch_stride, patch)
 #define PSALM_MSDA_G(GG)                                      \
   do {                                                        \
-    if (L == 3 && P == 4) PSALM_MSDA_LAUNCH(GG, 3, 4);        \
-    else if (L == 4 && P == 4) PSALM_MSDA_LAUNCH(GG, 4, 4);   \
-    else PSALM_MSDA_LAUNCH(GG, 0, 0);                         \
+    if (L == 3 && P == 4 && preload_ok) PSALM_MSDA_LAUNCH(GG, 3, 4);        \
+    else if (L == 4 && P == 4 && preload_ok) PSALM_MSDA_LAUNCH(GG, 4, 4);   \
+    else PSALM_MSDA_LAUNCH(GG, 0, 0);                                       \
   } while (0)
   PSALM_REQUIRE(L <= kMaxLevels && P <= 32, "msda: L=%d (max %d) or P=%d (max 32) too large", L, kMaxLevels, P);
   switch (G) {
@@ -480,6 +483,10 @@ static int launch_fused(const void* value, const void* ow, void* out, const int6
   PSALM_REQUIRE(G == 4 || G == 8, "msda_fused: D=%d unsupported (need D/%d in {4,8})", D, CH);
   PSALM_REQUIRE((long long)S * D < (1ll << 31), "msda_fused: S*D=%lld exceeds the 32-bit corner offsets", (long long)S * D);
   PSALM_REQUIRE((L == 3 || L == 4) && P == 4, "msda_fused: (L,P)=(%d,%d) unsupported", L, P);
+  // value is read and out written with 16-byte vectors, the (x, y) offset pairs of ow with one 2 * sizeof(TO) load
+  PSALM_REQUIRE(((reinterpret_cast<uintptr_t>(value) | reinterpret_cast<uintptr_t>(out)) % 16 == 0) &&
+                    reinterpret_cast<uintptr_t>(ow) % (2 * sizeof(TO)) == 0,
+                "msda_fused: value / out must be 16-byte aligned and ow %d-byte aligned", (int)(2 * sizeof(TO)));
   MsdaLevels lv;
   int tiles = 0;
   long long sumHW = 0;

@@ -283,7 +283,8 @@ def postproc_fused(logits, H, W, probsT=None, wq=None, negq=None, slot_query=Non
     """logits [Q,H4,W4] -> dict(sem_seg, ids, in_mask, inst_masks, stats [Q,5]) at output size (H, W).
     stats columns: count(x>0), sum(sigmoid*[x>0]), count(x>=0), panoptic area, panoptic intersection.
     crop = (Hp, Wp, oh, ow): up-sample to the padded size (Hp, Wp), crop to (oh, ow), resize to (H, W) (the reference's
-    sem_seg_postprocess flow) composed inside the kernel; None: (H, W) is the up-sampled size itself."""
+    sem_seg_postprocess flow) composed inside the kernel; None: (H, W) is the up-sampled size itself.
+    inst_masks of a slot_query entry -1 are not written."""
     import ctypes
     _chk(logits, "postproc_fused.logits")
     Q, H4, W4 = logits.shape
