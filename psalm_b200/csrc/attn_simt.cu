@@ -487,8 +487,10 @@ extern "C" int psalm_prefix_causal_attention(const void* qkv, const void* prefix
 extern "C" int psalm_rotary_inplace(void* qkv, const float* cos_t, const float* sin_t, int B, int T_, int nh,
                                     int hd, int rd, int dtype, void* stream) {
   PSALM_REQUIRE(qkv && cos_t && sin_t, "rotary: null pointer");
-  PSALM_REQUIRE(rd % 2 == 0 && rd <= hd, "rotary: bad rotary dim %d (head dim %d)", rd, hd);
-  if (dtype != PSALM_F32 && (rd / 2) % 8 == 0 && hd % 8 == 0) {
+  PSALM_REQUIRE(rd > 0 && rd % 2 == 0 && rd <= hd, "rotary: bad rotary dim %d (head dim %d)", rd, hd);
+  // the vector kernel makes 16-byte loads of qkv and cos / sin: a tensor with a storage offset takes the scalar kernel
+  const bool aligned = (((uintptr_t)qkv | (uintptr_t)cos_t | (uintptr_t)sin_t) & 15) == 0;
+  if (dtype != PSALM_F32 && (rd / 2) % 8 == 0 && hd % 8 == 0 && aligned) {
     const long long nv = (long long)B * T_ * 2 * nh * (rd / 16);
     const int vb = (int)((nv + 255) / 256 < 132 * 16 ? (nv + 255) / 256 : 132 * 16);
     if (dtype == PSALM_BF16) rotary_vec_kernel<__nv_bfloat16><<<vb > 0 ? vb : 1, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)qkv, cos_t, sin_t, B, T_, nh, hd, rd);

@@ -76,9 +76,20 @@ def window_attention(qkv, qkv_bias, rel_bias, B, H, W, C, nh, ws, shift):
 
 @_on_device
 def rotary_inplace(qkv, cos, sin, B, T, nh, hd, rd):
+    """Partial rotary embedding in place on q and k of qkv [B,T,3,nh,hd] (B*T*3*nh*hd elements): pairs (i, i + rd/2)
+    of the first rd dims rotate by cos/sin [T, rd/2] fp32, whose row t is the position of token t."""
     _chk(qkv, "rotary.qkv")
     _chk(cos, "rotary.cos")
     _chk(sin, "rotary.sin")
+    if not (0 < rd <= hd and rd % 2 == 0):
+        raise _lib.PsalmKernelError("rotary: rotary dim %d must be even and in (0, head dim %d]" % (rd, hd))
+    for t, n in ((cos, "cos"), (sin, "sin")):
+        if t.dtype != torch.float32 or tuple(t.shape) != (T, rd // 2):
+            raise _lib.PsalmKernelError("rotary.%s: expected fp32 [%d, %d], got %s %s"
+                                        % (n, T, rd // 2, t.dtype, tuple(t.shape)))
+    if qkv.numel() != B * T * 3 * nh * hd:
+        raise _lib.PsalmKernelError("rotary.qkv: %d elements, expected B*T*3*nh*hd = %d"
+                                    % (qkv.numel(), B * T * 3 * nh * hd))
     rc = _lib.lib().psalm_rotary_inplace(_lib.ptr(qkv), _lib.ptr(cos), _lib.ptr(sin), B, T, nh, hd, rd,
                                          _lib.dtype_code(qkv.dtype), _lib.stream_ptr(qkv.device))
     _lib.check(rc, "psalm_rotary_inplace")
